@@ -1,7 +1,7 @@
 """ctypes binding of libance_b200.so (the C ABI declared in include/ance_b200.h).
 
 There is no CPU fallback anywhere in this package: if the shared library is missing it is built
-(nvcc cross-compiles), and if that fails, or a compute entry point is called without an sm_100
+(nvcc cross-compiles), and if that fails, or a compute entry point is called without an sm_90
 device, the call raises.
 """
 from __future__ import annotations

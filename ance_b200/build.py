@@ -1,4 +1,4 @@
-"""In-tree build of libance_b200.so (sm_100a only) and of the CPU oracle library.
+"""In-tree build of libance_b200.so (sm_90a only) and of the CPU oracle library.
 
 nvcc cross-compiles without a GPU, so this runs in the CPU-only build container; the resulting
 ``ance_b200/lib/*.so`` files are git-ignored but travel to the GPU box with the snapshot.
@@ -19,7 +19,7 @@ OBJDIR = ROOT / "build" / "obj"
 LIB = LIBDIR / "libance_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-pthread",
     "--expt-relaxed-constexpr",
@@ -85,7 +85,7 @@ def _build_cuda_locked(force: bool, verbose: bool) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
     tmp = LIB.with_suffix(".so.tmp")
-    cmd = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
            "-Xcompiler", "-pthread"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

@@ -1,9 +1,9 @@
 // act16.cuh — the 16-bit storage format of encoder activations / weights as a compile-time trait.
 //
-// tcgen05 kind::f16 multiplies fp16 and bf16 operands at the same rate (fp32 accumulate either way); what differs is the
+// wgmma multiplies fp16 and bf16 operands at the same rate (fp32 accumulate either way); what differs is the
 // rounding of everything that is STORED between kernels: bf16 keeps 8 significant bits (unit roundoff 2^-9), fp16 keeps
 // 11 (2^-12).  The reference's forward is fp32 (model/models.py:149-157 under torch.no_grad, no autocast), so the encoder
-// defaults to fp16 storage, which brings the embeddings 8x closer to the reference at identical speed; bf16 stays
+// defaults to fp16 storage, which brings the embeddings 8x closer to the reference; bf16 stays
 // selectable for checkpoints whose activations leave the fp16 range (|x| > 65504 -> inf -> NaN embeddings, which
 // ance_encoder_check reports).
 #pragma once

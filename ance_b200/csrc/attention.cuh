@@ -7,13 +7,14 @@
 // (bias added in fp32 before the softmax), so an all-padding sequence gives the same finite
 // "softmax of the raw scores" the reference gives, not NaN.
 //
-// One work item = (128-token query tile, head); a persistent CTA per SM keeps two items in flight, one per
-// softmax warpgroup (see attention_kernel).  Per 128-key block of the same sequence:
-//   S = Q K^T          tcgen05.mma  M128 N128 K16 x4   (Q, K: TMA boxes of the [tokens, 3H] QKV buffer)
-//   softmax            4 warps per group, thread = query row: L <= 128 one trip to TMEM (row in registers: max, exp2),
-//                      L > 128 two passes per block with online rescaling;
+// One work item = (128-token query tile, head); a persistent CTA per SM walks its items while a TMA producer warp
+// streams Q / K / V up to kStages key blocks ahead.  Per 128-key block of the same sequence:
+//   S = Q K^T          wgmma m64n128k16 x (2 x 4)   (Q, K: TMA boxes of the [tokens, 3H] QKV buffer), written to a
+//                      shared fp32 score tile
+//   softmax            one warpgroup, thread = query row reading its row of the score tile: L <= 128 one pass (row in
+//                      registers: max, exp2), L > 128 two passes per block with online rescaling;
 //                      P written as 16-bit (FMT) into shared memory in the K-major SWIZZLE_128B layout
-//   O_blk = P V        tcgen05.mma  M128 N64 K16 x8    (V is the MN-major B operand)
+//   O_blk = P V        wgmma m64n64k16 x (2 x 8)    (V is the MN-major B operand), written over the score tile
 //   o = o*alpha + O_blk in registers; after the last block ctx = o / l  (16-bit)
 // Sequence lengths: a multiple of 128, or a divisor of 128 (then a tile holds 128/L sequences and
 // cross-sequence scores are excluded).  head_dim is fixed at 64 (BERT/RoBERTa-base).
@@ -49,18 +50,19 @@ struct Params {
 };
 
 struct Smem {
-  static constexpr int kGroups = 2;                            // softmax warpgroups, each with its own Q / S / P / O
-  static constexpr int kStages = 4;                            // (K, V) stages shared by both groups
+  static constexpr int kStages = 3;                            // (K, V) stages
   static constexpr int kTileBytes = kTile * kDh * 2;           // 16 KB: one 128 x 64 16-bit operand tile
   static constexpr int kQ = 0;
-  static constexpr int kKV = kQ + kGroups * kTileBytes;        // stage s: K at +0, V at +16 KB
-  static constexpr int kP = kKV + kStages * 2 * kTileBytes;    // per group 128 x 128 16-bit (two 64-key halves)
-  static constexpr int kBias = kP + kGroups * kTile * kTile * 2;   // per group 128 floats + 4 ballots
+  static constexpr int kKV = kQ + kTileBytes;                  // stage s: K at +0, V at +16 KB
+  static constexpr int kP = kKV + kStages * 2 * kTileBytes;    // 128 x 128 16-bit (two 64-key halves)
+  static constexpr int kSPitch = kTile + 4;                    // fp32 words per row of the score / output tile
+  static constexpr int kS = kP + kTile * kTile * 2;            // S (128 x 128 fp32), then O_blk (128 x 64) over it
+  static constexpr int kBias = kS + kTile * kSPitch * 4;       // 128 floats + 4 ballots
   static constexpr int kBiasStride = kTile * 4 + 16;
-  static constexpr int kBar = kBias + kGroups * kBiasStride;
-  // q_full[2] q_empty[2] kv_full[S] kv_empty[S] s[2] p[2] o[2]  + tmem ptr
-  static constexpr int kNumBars = 4 + 2 * kStages + 6;
-  static constexpr int kTotal = kBar + kNumBars * 8 + 16;
+  static constexpr int kBar = kBias + kBiasStride;
+  // q_full q_empty kv_full[S] kv_empty[S]
+  static constexpr int kNumBars = 2 + 2 * kStages;
+  static constexpr int kTotal = kBar + kNumBars * 8;
   static constexpr int kDynamic = kTotal + 1024;
   static_assert(kDynamic <= 232448, "attention smem exceeds 227 KB");
 };
@@ -68,14 +70,11 @@ struct Smem {
 // a running maximum above this is the score of an unmasked key: masked keys sit near -10000 log2(e) = -14427
 constexpr float kRealMax = -7000.0f;
 
-constexpr int kThreads = 384;   // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-7 softmax group 0, 8-11 softmax group 1
+constexpr int kThreads = 256;   // warp 0 TMA, 1-3 idle, 4-7 the softmax / MMA warpgroup
 
-// Persistent, one CTA per SM.  The CTA walks its work items w = blockIdx.x + n * gridDim.x; item n belongs to
-// softmax group n & 1, so two items are always in flight: while one group runs its softmax on the CUDA cores the
-// tensor core serves the other, and the TMA producer runs up to kStages key/value blocks ahead (the HBM latency
-// of a 48 KB Q/K/V fetch is longer than one item's arithmetic).  Blocks are issued in the interleaved order
-// (a,0) (b,0) (a,1) (b,1) ... for the item pair (a, b); producer, MMA issuer and both groups derive that order
-// from the same loop nest.
+// Persistent, one CTA per SM.  The CTA walks its work items w = blockIdx.x + n * gridDim.x; the TMA producer runs
+// up to kStages key/value blocks ahead (the HBM latency of a 48 KB Q/K/V fetch is longer than one item's
+// arithmetic); producer and warpgroup derive the block order from the same loop nest.
 // kPacked: L < 128, a tile holds 128/L sequences.  kSingle: L <= 128, one key block per item.
 // FMT: 16-bit format of Q / K / V, of the probabilities P and of the output (act16.cuh).
 template <bool kPacked, bool kSingle, uint32_t FMT>
@@ -85,14 +84,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Smem::kBar);
-  uint64_t* q_full = bars + 0;                       // [2]
-  uint64_t* q_empty = bars + 2;                      // [2]
-  uint64_t* kv_full = bars + 4;                      // [kStages]
-  uint64_t* kv_empty = bars + 4 + Smem::kStages;     // [kStages]
-  uint64_t* bar_s = bars + 4 + 2 * Smem::kStages;    // [2]
-  uint64_t* bar_p = bar_s + 2;                       // [2]
-  uint64_t* bar_o = bar_s + 4;                       // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + Smem::kNumBars);
+  uint64_t* q_full = bars + 0;
+  uint64_t* q_empty = bars + 1;
+  uint64_t* kv_full = bars + 2;                      // [kStages]
+  uint64_t* kv_empty = bars + 2 + Smem::kStages;     // [kStages]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.n_tokens + kTile - 1) / kTile;
@@ -102,119 +97,56 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmCTX);
-    for (int g = 0; g < Smem::kGroups; ++g) {
-      mbar_init(&q_full[g], 1);
-      mbar_init(&q_empty[g], 1);
-      mbar_init(&bar_s[g], 1);
-      mbar_init(&bar_p[g], 4);
-      mbar_init(&bar_o[g], 1);
-    }
+    mbar_init(q_full, 1);
+    mbar_init(q_empty, 4);          // the four warps of the warpgroup, after the last S of an item
     for (int s = 0; s < Smem::kStages; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
+      mbar_init(&kv_empty[s], 4);   // the four warps of the warpgroup, after the block's P V
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<1>(tmem_ptr_smem, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // group g: S at columns [128 g, 128 g + 128), O at [256 + 64 g, 256 + 64 g + 64)
 
   if (warp == 0) {
     // ================================ TMA producer ================================
     if (lane == 0) {
       Ring<Smem::kStages> kv;
-      uint32_t qc[2] = {0, 0};
-      for (int wa = blockIdx.x; wa < total_work; wa += 2 * gridDim.x) {
-        const int n_in_pair = (wa + static_cast<int>(gridDim.x) < total_work) ? 2 : 1;
+      uint32_t qc = 0;
+      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int tile = w / p.heads, h = w - tile * p.heads;
+        const int tok0 = tile * kTile;
+        const int kv_tok0 = (p.L >= kTile) ? (tok0 / p.L) * p.L : tok0;
         for (int j = 0; j < nkv; ++j) {
-          for (int g = 0; g < n_in_pair; ++g) {
-            const int w = wa + g * gridDim.x;
-            const int tile = w / p.heads, h = w - tile * p.heads;
-            const int tok0 = tile * kTile;
-            const int kv_tok0 = (p.L >= kTile) ? (tok0 / p.L) * p.L : tok0;
-            if (j == 0) {
-              mbar_wait(&q_empty[g], (qc[g] & 1) ^ 1, 10);
-              ++qc[g];
-              mbar_arrive_expect_tx(&q_full[g], Smem::kTileBytes);
-              tma_load_2d(smem + Smem::kQ + g * Smem::kTileBytes, &tmQKV, &q_full[g], h * kDh, tok0, kEvictFirst);
-            }
-            mbar_wait(&kv_empty[kv.stage], kv.phase ^ 1, 11);
-            mbar_arrive_expect_tx(&kv_full[kv.stage], 2 * Smem::kTileBytes);
-            uint8_t* st = smem + Smem::kKV + kv.stage * 2 * Smem::kTileBytes;
-            tma_load_2d(st, &tmQKV, &kv_full[kv.stage], p.hidden + h * kDh, kv_tok0 + j * kTile, kEvictNormal);
-            tma_load_2d(st + Smem::kTileBytes, &tmQKV, &kv_full[kv.stage], 2 * p.hidden + h * kDh, kv_tok0 + j * kTile,
-                        kEvictNormal);
-            kv.advance();
+          if (j == 0) {
+            mbar_wait(q_empty, (qc & 1) ^ 1, 10);
+            ++qc;
+            mbar_arrive_expect_tx(q_full, Smem::kTileBytes);
+            tma_load_2d(smem + Smem::kQ, &tmQKV, q_full, h * kDh, tok0, kEvictFirst);
           }
+          mbar_wait(&kv_empty[kv.stage], kv.phase ^ 1, 11);
+          mbar_arrive_expect_tx(&kv_full[kv.stage], 2 * Smem::kTileBytes);
+          uint8_t* st = smem + Smem::kKV + kv.stage * 2 * Smem::kTileBytes;
+          tma_load_2d(st, &tmQKV, &kv_full[kv.stage], p.hidden + h * kDh, kv_tok0 + j * kTile, kEvictNormal);
+          tma_load_2d(st + Smem::kTileBytes, &tmQKV, &kv_full[kv.stage], 2 * p.hidden + h * kDh, kv_tok0 + j * kTile,
+                      kEvictNormal);
+          kv.advance();
         }
       }
-    }
-  } else if (warp == 1) {
-    // ================================= MMA issuer =================================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_f16(kTile, kTile, FMT, 0, 0);  // Q K^T : both K-major
-      constexpr uint32_t idesc_o = make_idesc_f16(kTile, kDh, FMT, 0, 1);    // P V   : V is MN-major
-      Ring<Smem::kStages> kv;
-      uint32_t qc[2] = {0, 0}, bc[2] = {0, 0};
-      int prev_g = -1, prev_stage = 0;   // block whose S is issued and whose P V is still owed
-      auto issue_pv = [&](int g, int stage) {
-        mbar_wait(&bar_p[g], bc[g] & 1, 14);
-        ++bc[g];
-        tc_fence_after_sync();
-        const uint32_t sp = smem_u32(smem + Smem::kP + g * (kTile * kTile * 2));
-        const uint32_t sv = smem_u32(smem + Smem::kKV + stage * 2 * Smem::kTileBytes + Smem::kTileBytes);
-        const uint32_t tmem_O = tmem_base + 256 + g * kDh;
-#pragma unroll
-        for (int k = 0; k < kTile / 16; ++k) {
-          // A = P: keys [16k, 16k+16) live in 64-key half (k/4), 32 bytes per K step inside the span
-          const uint64_t adesc = make_desc_k_sw128(sp + (k >> 2) * (kTile * 128) + (k & 3) * 32);
-          // B = V (MN-major): 16 keys = two 8-row groups of 1024 bytes
-          const uint64_t bdesc = make_desc_mn_sw128(sv + k * 2048, kTile * 128, 1024);
-          umma_ss<1>(tmem_O, adesc, bdesc, idesc_o, k != 0);
-        }
-        umma_commit(&kv_empty[stage]);
-        umma_commit(&bar_o[g]);
-      };
-      for (int wa = blockIdx.x; wa < total_work; wa += 2 * gridDim.x) {
-        const int n_in_pair = (wa + static_cast<int>(gridDim.x) < total_work) ? 2 : 1;
-        for (int j = 0; j < nkv; ++j) {
-          for (int g = 0; g < n_in_pair; ++g) {
-            // S of group g may be overwritten only after the group's previous block published its P
-            if (prev_g == g) { issue_pv(prev_g, prev_stage); prev_g = -1; }
-            if (j == 0) { mbar_wait(&q_full[g], qc[g] & 1, 12); ++qc[g]; }
-            mbar_wait(&kv_full[kv.stage], kv.phase, 13);
-            tc_fence_after_sync();
-            const uint32_t sq = smem_u32(smem + Smem::kQ + g * Smem::kTileBytes);
-            const uint32_t sk = smem_u32(smem + Smem::kKV + kv.stage * 2 * Smem::kTileBytes);
-#pragma unroll
-            for (int k = 0; k < kDh / 16; ++k)
-              umma_ss<1>(tmem_base + g * kTile, make_desc_k_sw128(sq + k * 32), make_desc_k_sw128(sk + k * 32), idesc_s, k != 0);
-            umma_commit(&bar_s[g]);
-            if (j == nkv - 1) umma_commit(&q_empty[g]);
-            if (prev_g >= 0) issue_pv(prev_g, prev_stage);
-            prev_g = g;
-            prev_stage = kv.stage;
-            kv.advance();
-          }
-        }
-      }
-      if (prev_g >= 0) issue_pv(prev_g, prev_stage);
     }
   } else if (warp >= 4) {
     // =============================== softmax / output ==============================
-    const int g = (warp - 4) >> 2;             // softmax group
-    const int quad = warp & 3;                 // TMEM lane quarter this warp may read
+    const int quad = warp & 3;                 // 32-row quarter of the tile this warp owns
     const int row = quad * 32 + lane;          // query row inside the tile
-    const uint32_t lane_sel = static_cast<uint32_t>(quad * 32) << 16;
-    const uint32_t tmem_S = tmem_base + g * kTile;
-    const uint32_t tmem_O = tmem_base + 256 + g * kDh;
-    uint8_t* sP = smem + Smem::kP + g * (kTile * kTile * 2);
-    float* sbias = reinterpret_cast<float*>(smem + Smem::kBias + g * Smem::kBiasStride);
+    uint8_t* sP = smem + Smem::kP;
+    float* sS = reinterpret_cast<float*>(smem + Smem::kS);
+    const uint32_t srow = smem_u32(sS) / 4u + static_cast<uint32_t>(row * Smem::kSPitch);   // this row, word address
+    float* sbias = reinterpret_cast<float*>(smem + Smem::kBias);
     unsigned* smask = reinterpret_cast<unsigned*>(sbias + kTile);  // per-warp ballots of masked keys
-    const int bar_id = 1 + g;
+    const int bar_id = 1;
+    const uint32_t sq = smem_u32(smem + Smem::kQ);
+    const uint32_t sp = smem_u32(sP);
+    Ring<Smem::kStages> kv;
+    uint32_t qc = 0;
     // additive key bias of block (w2, j2) for key `row` of that block (fetched one block ahead of its use)
     auto load_bias = [&](int w2, int j2) -> float {
       if (w2 >= total_work) return 0.f;
@@ -230,10 +162,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
         *reinterpret_cast<uint4*>(rowp + ch * 16) = make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
       }
     };
-    uint32_t it = 0;
-    const int w_first = blockIdx.x + g * gridDim.x;
-    float bv = load_bias(w_first, 0);
-    for (int w = w_first; w < total_work; w += 2 * gridDim.x) {
+    float bv = load_bias(blockIdx.x, 0);
+    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       const int tile = w / p.heads, h = w - tile * p.heads;
       const int tok0 = tile * kTile;
       const bool varlen = kPacked && p.row_lo != nullptr;
@@ -249,9 +179,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
 #pragma unroll
         for (int i = 0; i < kDh; ++i) o[i] = 0.f;
       }
-      for (int j = 0; j < nkv; ++j, ++it) {
-        // key bias of this block -> smem (the previous block's readers are past their last use: they all arrived
-        // on bar_p before the PV MMA whose completion this thread has waited for)
+      for (int j = 0; j < nkv; ++j) {
+        // key bias of this block -> smem (the previous block's readers are past their last use: they all passed
+        // the barrier after the P V of that block)
         sbias[row] = bv;
         {
           const unsigned mk = __ballot_sync(0xffffffffu, bv < 0.f);
@@ -259,7 +189,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
         }
         if (row == 0) bulk_wait_read_all();   // the previous item's output tile has left sP
         named_bar_sync(bar_id, kTile);
-        bv = (j + 1 < nkv) ? load_bias(w, j + 1) : load_bias(w + 2 * gridDim.x, 0);
+        bv = (j + 1 < nkv) ? load_bias(w, j + 1) : load_bias(w + gridDim.x, 0);
         // Per 32-key chunk, warp-uniform:  0 = every p is exactly 0 (keys of another packed sequence, or all keys
         // masked while the row has an unmasked key somewhere: exp2(-10000 log2e + s - m) flushes to zero, as
         // exp(-10000 + s - m) does in the reference's fp32 softmax),  1 = no key masked (no bias term),  2 = general.
@@ -284,16 +214,41 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
           for (int c = 0; c < 4; ++c)
             st[c] = !own[c] ? 0 : (mk[c] == 0xffffffffu && skip_ok) ? 0 : (mk[c] == 0u && !(kPacked && p.L < 32)) ? 1 : 2;
         }
-        mbar_wait(&bar_s[g], it & 1, 15);
-        tc_fence_after_sync();
+        // S = Q K^T -> the score tile
+        if (j == 0) mbar_wait(q_full, qc & 1, 12);
+        mbar_wait(&kv_full[kv.stage], kv.phase, 13);
+        const uint32_t sk = smem_u32(smem + Smem::kKV + kv.stage * 2 * Smem::kTileBytes);
+        {
+          float s0[kTile / 2], s1[kTile / 2];
+#pragma unroll
+          for (int i = 0; i < kTile / 2; ++i) s0[i] = s1[i] = 0.f;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kDh / 16; ++k) {
+            const uint64_t bdesc = make_desc_k_sw128(sk + k * 32);
+            wgmma_n128<FMT, 0>(s0, make_desc_k_sw128(sq + k * 32), bdesc, 1u);
+            wgmma_n128<FMT, 0>(s1, make_desc_k_sw128(sq + 64 * 128 + k * 32), bdesc, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(s0);
+          wgmma_fence_regs(s1);
+          acc_store_frag(sS, Smem::kSPitch, 0, 0, s0);
+          acc_store_frag(sS, Smem::kSPitch, 64, 0, s1);
+        }
+        if (j == nkv - 1) {   // the item's last read of Q
+          __syncwarp();
+          if (lane == 0) mbar_arrive(q_empty);
+          ++qc;
+        }
+        named_bar_sync(bar_id, kTile);   // every row of S is in the tile
         float rsum, alpha = 1.f, m_new;
         bool all_skip = false;
         if constexpr (kSingle) {
-          // one key block per item: the whole score row lives in registers, one trip to TMEM
+          // one key block per item: the whole score row lives in registers, one read of the score tile
           uint32_t v[kTile];
 #pragma unroll
-          for (int c = 0; c < kTile; c += 32) tmem_ld_32x32b_x32p(tmem_S + lane_sel + c, v + c);
-          tmem_ld_wait();
+          for (int c = 0; c < kTile; c += 32) acc_ld_x32(srow + c, v + c);
           float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
           if (plain) {   // max of the raw scores: scale > 0 commutes with max
 #pragma unroll
@@ -358,8 +313,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
                 for (int i = 0; i < 16; ++i) pk[i] = 0u;
               } else {
                 uint32_t v[32];
-                tmem_ld_32x32b_x32(tmem_S + lane_sel + c, v);
-                tmem_ld_wait();
+                acc_ld_x32(srow + c, v);
                 if (sc_ == 1) {
 #pragma unroll
                   for (int i = 0; i < 32; i += 2) {
@@ -405,7 +359,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
               }
             } else {
               float dummy;
-              exp_pass(m_run, dummy);   // (writes the zero P tile; no TMEM reads: every chunk state is 0)
+              exp_pass(m_run, dummy);   // (writes the zero P tile; no score reads: every chunk state is 0)
             }
           } else {
             // first block of an item (or no real key seen yet): pass 1 = row max (of the raw scores when `plain`:
@@ -417,8 +371,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
                 const int sc_ = (stb >> (c >> 4)) & 3;
                 if (sc_ == 0) continue;
                 uint32_t v[32];
-                tmem_ld_32x32b_x32(tmem_S + lane_sel + c, v);
-                tmem_ld_wait();
+                acc_ld_x32(srow + c, v);
                 if (plain) {
 #pragma unroll
                   for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]));
@@ -438,12 +391,34 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
           }
         }
         fence_proxy_async_smem();
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_p[g]);
-        // O_blk
-        mbar_wait(&bar_o[g], it & 1, 16);
-        tc_fence_after_sync();
+        named_bar_sync(bar_id, kTile);   // P complete; every read of S is done
+        // O_blk = P V -> the same tile
+        {
+          const uint32_t sv = sk + Smem::kTileBytes;
+          float o0[kDh / 2], o1[kDh / 2];
+#pragma unroll
+          for (int i = 0; i < kDh / 2; ++i) o0[i] = o1[i] = 0.f;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kTile / 16; ++k) {
+            // A = P: keys [16k, 16k+16) live in 64-key half (k/4), 32 bytes per K step inside the span
+            const uint32_t pa = sp + (k >> 2) * (kTile * 128) + (k & 3) * 32;
+            // B = V (MN-major): 16 keys = two 8-row groups of 1024 bytes
+            const uint64_t bdesc = make_desc_mn_sw128(sv + k * 2048, kTile * 128, 1024);
+            wgmma_n64<FMT, 1>(o0, make_desc_k_sw128(pa), bdesc, 1u);
+            wgmma_n64<FMT, 1>(o1, make_desc_k_sw128(pa + 64 * 128), bdesc, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(o0);
+          wgmma_fence_regs(o1);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&kv_empty[kv.stage]);
+          kv.advance();
+          acc_store_frag(sS, Smem::kSPitch, 0, 0, o0);
+          acc_store_frag(sS, Smem::kSPitch, 64, 0, o1);
+        }
+        named_bar_sync(bar_id, kTile);   // every row of O_blk is in the tile
         if constexpr (kSingle) {
           l_run = rsum;
         } else {
@@ -451,12 +426,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
 #pragma unroll
             for (int c = 0; c < kDh; c += 32) {
               uint32_t v[32];
-              tmem_ld_32x32b_x32(tmem_O + lane_sel + c, v);
-              tmem_ld_wait();
+              acc_ld_x32(srow + c, v);
 #pragma unroll
               for (int i = 0; i < 32; ++i) o[c + i] = fmaf(o[c + i], alpha, __uint_as_float(v[i]));
             }
-            tc_fence_before_sync();
             l_run = fmaf(l_run, alpha, rsum);
             m_run = m_new;
           }
@@ -467,10 +440,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
         const float inv = 1.0f / l_run;
         if constexpr (kSingle) {
           uint32_t v[kDh];
-          tmem_ld_32x32b_x32p(tmem_O + lane_sel, v);
-          tmem_ld_32x32b_x32p(tmem_O + lane_sel + 32, v + 32);
-          tmem_ld_wait();
-          tc_fence_before_sync();
+          acc_ld_x32(srow, v);
+          acc_ld_x32(srow + 32, v + 32);
 #pragma unroll
           for (int i = 0; i < kDh; ++i) o[i] = __uint_as_float(v[i]);
         }
@@ -494,9 +465,6 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
     if (row == 0) bulk_wait_read_all();
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 }  // namespace attn

@@ -51,7 +51,7 @@ void prof_end(int cls, cudaStream_t st) {
 
 }  // namespace ance
 
-extern "C" const char* ance_version(void) { return "ance_b200 0.1 (sm_100a)"; }
+extern "C" const char* ance_version(void) { return "ance_b200 0.1 (sm_90a)"; }
 extern "C" const char* ance_last_error(void) { return ance::g_err; }
 extern "C" int64_t ance_launch_count(void) { return ance::g_launches.load(); }
 
@@ -84,7 +84,7 @@ namespace {
 template <int BN, int STAGES, int CG, uint32_t FMT>
 int run_dbg(const void* A, const void* B, int M, int N, int K, const float* bias, const void* R, int act, void* C,
             float* C32, cudaStream_t st) {
-  constexpr int EW = (BN >= 128) ? 8 : 4;
+  constexpr int EW = 4;
   using Ep = gemm::EpStore<BN, EW>;
   CUtensorMap tmA, tmB;
   if (!tc05_host::make_tmap_2d_16b(&tmA, A, M, K, K, gemm::BM) ||
@@ -120,11 +120,11 @@ template <uint32_t FMT>
 int dispatch_dbg(int variant, const void* A, const void* B, int M, int N, int K, const float* bias, const void* R,
                  int act, void* C, float* C32, cudaStream_t st) {
   switch (variant) {
-    case 0: return run_dbg<256, 4, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
-    case 1: return run_dbg<128, 6, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
-    case 2: return run_dbg<256, 6, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
-    case 3: return run_dbg<128, 8, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
-    case 4: return run_dbg<64, 8, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 0: return run_dbg<128, 4, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 1: return run_dbg<128, 3, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 2: return run_dbg<128, 4, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 3: return run_dbg<64, 6, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 4: return run_dbg<64, 6, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
     default: ance::set_error("ance_dbg_gemm: unknown variant %d", variant); return ANCE_ERR_INVALID;
   }
 }

@@ -1,11 +1,11 @@
-// encoder.cu — BERT/RoBERTa-base dual-encoder forward on sm_100a.
+// encoder.cu — BERT/RoBERTa-base dual-encoder forward on sm_90a.
 //
 // Replaces the library calls behind the reference's
 //   model/models.py:149-157  RobertaDot_NLL_LN.query_emb/body_emb  (HF RobertaModel -> CLS -> embeddingHead -> norm)
 //   model/models.py:165-199  MultiChunk body_emb (caller reshapes [B,2048] -> [4B,512]; token 0 of each chunk)
 //   model/models.py:223-259  BiEncoder / HFBertEncoder (CLS of the last layer)
 // Per layer (SURVEY.md §2.3 K1-K7):
-//   QKV  = X Wqkv^T + b                       tcgen05 GEMM (gemm_core.cuh), bias epilogue
+//   QKV  = X Wqkv^T + b                       wgmma GEMM (gemm_core.cuh), bias epilogue
 //   CTX  = softmax(QK^T/8 + mask) V           attention.cuh
 //   T    = CTX Wo^T + b + X ; X1 = LN(T)      GEMM with bias+residual epilogue, then ln_rows_kernel
 //   F    = gelu_erf(X1 W1^T + b1)             GEMM with bias+GELU epilogue
@@ -294,7 +294,7 @@ __global__ void gather_rows_f32_kernel(const uint16_t* __restrict__ X, size_t ro
 
 // Same arithmetic again (bit-identical), holding the rows PACKED: kB x NV uint4 registers instead of kB x NV x 8 floats; the
 // three passes (sum, variance, normalise) unpack on the fly.  ~56 instead of 83 registers per thread -> 4 instead of 3
-// resident blocks per SM (ncu of the float form: 21 % of the warp slots active, latency-bound at 0.6-0.8 of the HBM roof).
+// resident blocks per SM (the float form is latency-bound, well below the HBM roof).
 template <int NV, int kB, uint32_t FMT>
 __global__ void __launch_bounds__(256, 4) ln_rows_packed_kernel(const uint16_t* __restrict__ in, size_t in_ld, int n_rows, int H,
                                                                 const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -460,15 +460,13 @@ uint16_t* upload_16(ance_encoder* e, const float* h, size_t n) {
 }
 
 // one GEMM of the forward: C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ R)
-// cta_group::2: 256 x 256 tile per CTA pair.  EW = 8 epilogue warps (two 128-column groups, 6 smem stages) or EW = 16
-// (four 64-column groups, each with its own staging slab, 5 stages): with 16 a tile's epilogue is ONE
-// LDTM -> math -> TMA-store round per warp instead of two in sequence.  Measured at 592 x 128 (ms per forward, 8 -> 16):
-// FFN-up (GELU) 4.15 -> 3.62, out-proj 1.15 -> 1.06, but QKV 2.55 -> 2.90 and FFN-down 2.81 -> 2.90: the heavy / short-K
-// epilogues want the shorter chain, the light ones the deeper operand pipeline.
-template <int EW, int STAGES, uint32_t FMT>
-int linear_cfg(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
-               const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls, size_t ldr) {
-  constexpr int BN = 256, CG = 2;
+// 128 x 128 tile per CTA (the wgmma warpgroup holds the whole tile in registers: 128 fp32 accumulators per thread),
+// 4 operand stages, 4 epilogue warps reading the shared accumulator tile while the next tile is computed.
+template <uint32_t FMT>
+int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
+           const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls = ance::kClsGemm,
+           size_t ldr = 0) {
+  constexpr int BN = 128, CG = 1, EW = 4, STAGES = 4;
   using Ep = gemm::EpStore<BN, EW, FMT>;
   CUtensorMap tmA, tmB;
   if (!tc05_host::make_tmap_2d_16b(&tmA, A, M, K, lda, gemm::BM) || !tc05_host::make_tmap_2d_16b(&tmB, W, N, K, K, BN / CG)) {
@@ -494,7 +492,7 @@ int linear_cfg(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, i
   p.ldc = N;
   p.ldc32 = N;
   p.ldr = static_cast<int>(ldr);
-  // 2 = logistic form (|err| <= 3.7e-6, FFN-up 3.66 -> 3.49 ms per forward, A/B on one box), 1 = erfc form (|err| <= 7e-7)
+  // 2 = logistic form (|err| <= 3.7e-6), 1 = erfc form (|err| <= 7e-7)
   static const int gelu_form = getenv("ANCE_B200_GELU") ? atoi(getenv("ANCE_B200_GELU")) : 2;
   p.act = act ? gelu_form : 0;
   {
@@ -505,18 +503,7 @@ int linear_cfg(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, i
   return ANCE_OK;
 }
 
-template <uint32_t FMT>
-int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
-           const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls = ance::kClsGemm,
-           size_t ldr = 0) {
-  bool short_chain = (act != 0) || (R != nullptr && K <= 1024);   // FFN-up, out-proj
-  static const char* force = getenv("ANCE_B200_EPI_MASK");   // tuning aid: bit per GEMM class (qkv, out, ffn1, ffn2)
-  if (force && cls >= ance::kClsGemmQkv && cls <= ance::kClsGemmFfn2) short_chain = (atoi(force) >> (cls - ance::kClsGemmQkv)) & 1;
-  if (short_chain) return linear_cfg<16, 5, FMT>(A, lda, M, W, N, K, bias, R, act, C, C32, st, cls, ldr);
-  return linear_cfg<8, 6, FMT>(A, lda, M, W, N, K, bias, R, act, C, C32, st, cls, ldr);
-}
-
-int g_ln_rows_per_warp = 2;   // ance_encoder_set_param("ln_rows_per_warp"): 1.58 -> 1.25 ms per forward at 592 x 128 (4: 1.65)
+int g_ln_rows_per_warp = 2;   // ance_encoder_set_param("ln_rows_per_warp")
 
 template <uint32_t FMT>
 int layer_norm(const void* in, bool in_f32, size_t in_ld, int rows, int H, const float* g, const float* b, float eps,
@@ -680,8 +667,10 @@ extern "C" int ance_encoder_create(const ance_encoder_config* cfg, const ance_en
     int major = 0;
     ANCE_CUDA(cudaGetDevice(&dev));
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    if (major != 10) {
-      ance::set_error("device %d has compute capability %d.x; libance_b200 is built for sm_100a only (no CPU fallback)", dev, major);
+    int minor = 0;
+    cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+    if (major != 9 || minor != 0) {
+      ance::set_error("device %d has compute capability %d.%d; libance_b200 is built for sm_90a only (no CPU fallback)", dev, major, minor);
       return ANCE_ERR_CUDA;
     }
   }
@@ -793,7 +782,7 @@ namespace {
 // fullest tile that still has room for it (all tiles of the chunk stay open, so this packs almost as well as an offline
 // pass).  Stops at the first sequence that fits nowhere, or at max_seqs.  Returns the number of sequences placed.
 // align: every sequence starts at a multiple of `align` rows of its tile (its slot is padded up to a multiple).  With
-// align = 16 — the K step of a 16-bit tcgen05.mma — the P*V accumulation and the softmax row sum of a sequence group their
+// align = 16 — the K step of a 16-bit wgmma — the P*V accumulation and the softmax row sum of a sequence group their
 // terms exactly as they do at offset 0, so its embedding does not depend on what else is in the tile and equals the dense
 // forward's bit for bit; align = 1 packs ~12 % more real tokens per tile.
 int pack_chunk(const int32_t* lens, int first, int B, int cap_tiles, int max_seqs, int align, std::vector<int32_t>& row0,

@@ -1,19 +1,21 @@
-// gemm_core.cuh — the one tcgen05 mainloop of this repo.
+// gemm_core.cuh — the one wgmma mainloop of this repo.
 //
-//   D[M,N] = A[M,K] * B[N,K]^T        A, B: 16-bit (bf16 or fp16), K-major, fp32 accumulate in TMEM
+//   D[M,N] = A[M,K] * B[N,K]^T        A, B: 16-bit (bf16 or fp16), K-major, fp32 accumulate
 //
 // Used by (i) the encoder's linear layers (x * W^T, W stored [out,in] as in the checkpoint) and
 // (ii) the coarse pass of the flat inner-product search (Q * P^T).  The two differ only in the
 // epilogue functor `Ep` (bias/GELU/residual store vs. per-query running top-k).
 //
 // Structure (one CTA per SM, persistent, warp-specialised):
-//   warp 0   : TMA producer   — streams 128x64 A and (BN/CG)x64 B tiles through a STAGES-deep smem ring
-//   warp 1   : MMA issuer     — one thread issues tcgen05.mma (M = 128*CG, N = BN, K = 16) x 4 per k-block
-//   warp 2   : TMEM allocator — 2 accumulator stages of BN fp32 columns each (double buffered)
-//   warp 3   : idle
-//   warps 4+ : epilogue       — tcgen05.ld the accumulator, run Ep, release the TMEM stage
-// CG = 2 pairs two CTAs (cluster 2x1x1) on one 256-row tile: each CTA loads its own 128 A rows and
-// half of the B rows, the leader CTA issues the MMAs, commits are multicast to both CTAs.
+//   warp 0     : TMA producer  — streams 128x64 A and BNx64 B tiles through a STAGES-deep smem ring
+//   warps 4-7  : MMA warpgroup — wgmma m64nBNk16 (two per 16-wide K step: rows 0-63 and 64-127), fp32
+//                accumulators in registers; at the end of a tile they are written to a shared-memory
+//                accumulator tile (row-major fp32) and the warpgroup moves on to the next tile
+//   warps 8+   : epilogue      — read the accumulator tile (thread = row), run Ep, release the tile
+// The register accumulators and the shared tile form a two-deep pipeline: the epilogue of tile i runs
+// under the mainloop of tile i + 1.
+// CG = 2 pairs two CTAs (cluster 2x1x1) on one 256-row tile: each CTA computes its own 128 A rows,
+// the BN B rows are shared — each CTA loads half of them and multicasts it into both CTAs' rings.
 //
 // A "work item" is (m_blk, split): one M tile swept over a contiguous range of N blocks.  Plain
 // GEMMs use one N block per work item; the search sweeps thousands, carrying top-k state.
@@ -26,7 +28,7 @@ using namespace tc05;
 
 constexpr int BM = 128;  // rows per CTA
 constexpr int BK = 64;   // 64 x 16-bit = one 128-byte swizzle span
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 
 struct WorkShape {
   int M, N, K;
@@ -61,7 +63,7 @@ struct EpiCtx {
   int m_blk, split;
   int nb0, nb1;     // n-block range of this work item
   int row0;         // first global row of this CTA's 128-row tile
-  int quad;         // TMEM lane quadrant of this warp (warp_idx % 4)
+  int quad;         // 32-row quarter of the tile this warp reads (warp_idx % 4)
   int epi_warp;     // 0 .. EPI_WARPS-1
   int lane;
   int work_seq;     // how many work items this CTA has processed before this one
@@ -71,34 +73,43 @@ struct EpiCtx {
 template <int BN, int STAGES, int CG, int EP_SMEM = 0>
 struct SmemPlan {
   static constexpr int kABytes = BM * BK * 2;
-  static constexpr int kBRows = BN / CG;
-  static constexpr int kBBytes = kBRows * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;            // the whole B tile in every CTA of the cluster
+  static constexpr int kBHalfRows = BN / CG;              // rows of it this CTA loads (and multicasts when CG = 2)
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kRingBytes = STAGES * kStageBytes;
-  static constexpr int kEpOffset = kRingBytes;
-  static constexpr int kBarOffset = kRingBytes + EP_SMEM;
-  // full[STAGES] empty[STAGES] tmem_full[2] tmem_empty[2] + tmem ptr
-  static constexpr int kBarBytes = (2 * STAGES + 4) * 8 + 16;
+  static constexpr int kAccPitch = BN + 4;                // fp32 words per accumulator row
+  static constexpr int kAccOffset = kRingBytes;
+  static constexpr int kAccBytes = (BM * kAccPitch * 4 + 1023) / 1024 * 1024;
+  static constexpr int kEpOffset = kAccOffset + kAccBytes;
+  static constexpr int kBarOffset = kEpOffset + EP_SMEM;
+  // full[STAGES] empty[STAGES] acc_full acc_empty
+  static constexpr int kBarBytes = (2 * STAGES + 2) * 8;
   static constexpr int kTotal = kBarOffset + kBarBytes;
   static constexpr int kDynamicBytes = kTotal + 1024;  // slack for manual 1024-B alignment
+  static_assert(kDynamicBytes <= 232448, "GEMM shared memory exceeds 227 KB");
 };
 
+template <uint32_t FMT, int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (BN == 128) wgmma_n128<FMT, 0>(d, adesc, bdesc, accumulate);
+  else wgmma_n64<FMT, 0>(d, adesc, bdesc, accumulate);
+}
+
 template <class Ep, int BN, int STAGES, int CG, int EPI_WARPS, uint32_t FMT>
-__global__ void __launch_bounds__(128 + 32 * EPI_WARPS, 1)
+__global__ void __launch_bounds__(256 + 32 * EPI_WARPS, 1)
 tc05_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const WorkShape ws, const __grid_constant__ typename Ep::Params ep) {
-  static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "BN");
+  static_assert(BN == 64 || BN == 128, "BN");
   static_assert(CG == 1 || CG == 2, "CG");
   using Plan = SmemPlan<BN, STAGES, CG, Ep::kSmemBytes>;
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* acc_tile = reinterpret_cast<float*>(smem + Plan::kAccOffset);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Plan::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* afull_bar = empty_bar + STAGES;
+  uint64_t* aempty_bar = afull_bar + 1;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -113,20 +124,14 @@ tc05_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);   // the leader CTA's producer arrives once and expects both CTAs' bytes
-      mbar_init(&empty_bar[s], 1);  // one tcgen05.commit
+      mbar_init(&full_bar[s], 1);        // this CTA's producer arrives once; A + both B halves complete on it
+      mbar_init(&empty_bar[s], 4 * CG);  // every MMA warp of every CTA that multicasts into this stage
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], CG * EPI_WARPS);
-    }
+    mbar_init(afull_bar, 4);
+    mbar_init(aempty_bar, EPI_WARPS);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<CG>(tmem_ptr_smem, kTmemCols);
-  tc_fence_before_sync();
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == 0) {
     // ===================================== TMA producer =====================================
@@ -142,74 +147,88 @@ tc05_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (ws.pace != nullptr && leader && ((nb - nb0) & 7) == 0)
             pace_wait(ws.pace, ws.pace_window, cluster_id, num_clusters, ws.pace_stride,
                       ((w - cluster_id) / num_clusters) * ws.num_n_blks + (nb - nb0));
-          const int b_row = nb * BN + (int)cta_rank * Plan::kBRows;
+          const int b_row = nb * BN + (int)cta_rank * Plan::kBHalfRows;
           for (int kb = 0; kb < num_kb; ++kb) {
+            // CG = 2: the stage is free only when the MMA warps of BOTH CTAs have released it (each of them arrives
+            // on the empty barrier of both), since this CTA's half of B lands in the peer's ring too.
             mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1, 1);
             uint8_t* sa = smem + ring.stage * Plan::kStageBytes;
-            uint8_t* sb = sa + Plan::kABytes;
-            if constexpr (CG == 1) {
-              mbar_arrive_expect_tx(&full_bar[ring.stage], Plan::kStageBytes);
-              tma_load_2d(sa, &tmA, &full_bar[ring.stage], kb * BK, a_row, hint_a);
-              tma_load_2d(sb, &tmB, &full_bar[ring.stage], kb * BK, b_row, hint_b);
-            } else {
-              // Both CTAs' TMA bytes complete on the LEADER's barrier; only the leader arrives on it.  The
-              // peer cannot run a phase ahead: it refills a stage only after the MMA that consumed it
-              // (multicast commit on its own empty barrier).
-              if (leader) mbar_arrive_expect_tx(&full_bar[ring.stage], 2 * Plan::kStageBytes);
-              tma_load_2d_2sm(sa, &tmA, &full_bar[ring.stage], kb * BK, a_row, hint_a);
-              tma_load_2d_2sm(sb, &tmB, &full_bar[ring.stage], kb * BK, b_row, hint_b);
-            }
+            uint8_t* sb = sa + Plan::kABytes + cta_rank * (Plan::kBHalfRows * 128);
+            mbar_arrive_expect_tx(&full_bar[ring.stage], Plan::kStageBytes);
+            tma_load_2d(sa, &tmA, &full_bar[ring.stage], kb * BK, a_row, hint_a);
+            if constexpr (CG == 1) tma_load_2d(sb, &tmB, &full_bar[ring.stage], kb * BK, b_row, hint_b);
+            else tma_load_2d_multicast(sb, &tmB, &full_bar[ring.stage], kb * BK, b_row, 0x3, hint_b);
             ring.advance();
           }
         }
       }
       if (ws.pace != nullptr && leader) *reinterpret_cast<volatile int*>(ws.pace + cluster_id) = 0x7fffffff;   // done: never the slowest
     }
-  } else if (warp == 1) {
-    // ====================================== MMA issuer ======================================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = make_idesc_f16(BM * CG, BN, FMT, 0, 0);
-      Ring<STAGES> ring;
-      Ring<2> acc;
-      for (int w = cluster_id; w < total_work; w += num_clusters) {
-        const int m_blk = w / ws.n_splits, split = w - m_blk * ws.n_splits;
-        const int nb0 = split * ws.n_blks_per_split;
-        const int nb1 = min(nb0 + ws.n_blks_per_split, ws.num_n_blks);
-        for (int nb = nb0; nb < nb1; ++nb) {
-          mbar_wait(&tempty_bar[acc.stage], acc.phase ^ 1, 2);
-          tc_fence_after_sync();
-          const uint32_t tmem_d = tmem_base + acc.stage * BN;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[ring.stage], ring.phase, 3);
-            tc_fence_after_sync();
-            const uint32_t sa = smem_u32(smem + ring.stage * Plan::kStageBytes);
-            const uint32_t sb = sa + Plan::kABytes;
+  } else if (warp >= 4 && warp < 8) {
+    // ===================================== MMA warpgroup ====================================
+    Ring<STAGES> ring;
+    uint32_t acc_phase = 0;
+    auto release = [&](int stage) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[stage]);
+        if constexpr (CG == 2) mbar_arrive_cluster(&empty_bar[stage], cta_rank ^ 1u);
+      }
+    };
+    for (int w = cluster_id; w < total_work; w += num_clusters) {
+      const int m_blk = w / ws.n_splits, split = w - m_blk * ws.n_splits;
+      const int nb0 = split * ws.n_blks_per_split;
+      const int nb1 = min(nb0 + ws.n_blks_per_split, ws.num_n_blks);
+      (void)m_blk;
+      for (int nb = nb0; nb < nb1; ++nb) {
+        float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t adesc = make_desc_k_sw128(sa + k * UMMA_K * 2);
-              const uint64_t bdesc = make_desc_k_sw128(sb + k * UMMA_K * 2);
-              umma_ss<CG>(tmem_d, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-            if constexpr (CG == 1) umma_commit(&empty_bar[ring.stage]);
-            else umma_commit_2sm(&empty_bar[ring.stage], 0x3);
-            ring.advance();
+        for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+        int prev_stage = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&full_bar[ring.stage], ring.phase, 3);
+          const uint32_t sa = smem_u32(smem + ring.stage * Plan::kStageBytes);
+          const uint32_t sb = sa + Plan::kABytes;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / MMA_K; ++k) {
+            const uint64_t bdesc = make_desc_k_sw128(sb + k * MMA_K * 2);
+            wgmma_tile<FMT, BN>(acc0, make_desc_k_sw128(sa + k * MMA_K * 2), bdesc, 1u);
+            wgmma_tile<FMT, BN>(acc1, make_desc_k_sw128(sa + 64 * 128 + k * MMA_K * 2), bdesc, 1u);
           }
-          if constexpr (CG == 1) umma_commit(&tfull_bar[acc.stage]);
-          else umma_commit_2sm(&tfull_bar[acc.stage], 0x3);
-          acc.advance();
+          wgmma_commit();
+          // the previous k block's wgmmas have finished reading their stage once at most one group is in flight
+          wgmma_wait<1>();
+          wgmma_fence_regs(acc0);
+          wgmma_fence_regs(acc1);
+          if (prev_stage >= 0) release(prev_stage);
+          prev_stage = ring.stage;
+          ring.advance();
         }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        if (prev_stage >= 0) release(prev_stage);
+        // hand the tile to the epilogue once it has finished reading the previous one
+        mbar_wait(aempty_bar, acc_phase ^ 1, 2);
+        acc_store_frag(acc_tile, Plan::kAccPitch, 0, 0, acc0);
+        acc_store_frag(acc_tile, Plan::kAccPitch, 64, 0, acc1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(afull_bar);
+        acc_phase ^= 1;
       }
     }
-  } else if (warp >= 4) {
+  } else if (warp >= 8) {
     // ======================================= epilogue =======================================
     Ep epi;
     EpiCtx cx;
     cx.quad = warp & 3;
-    cx.epi_warp = warp - 4;
+    cx.epi_warp = warp - 8;
     cx.lane = lane;
     cx.work_seq = 0;
     cx.ep_smem = smem + Plan::kEpOffset;
-    Ring<2> acc;
+    uint32_t acc_phase = 0;
+    const uint32_t tacc = smem_u32(acc_tile) / 4u + static_cast<uint32_t>((cx.quad * 32 + lane) * Plan::kAccPitch);
     for (int w = cluster_id; w < total_work; w += num_clusters, ++cx.work_seq) {
       cx.m_blk = w / ws.n_splits;
       cx.split = w - cx.m_blk * ws.n_splits;
@@ -218,26 +237,19 @@ tc05_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       cx.row0 = (cx.m_blk * CG + (int)cta_rank) * BM;
       epi.begin_work(ep, ws, cx);
       for (int nb = cx.nb0; nb < cx.nb1; ++nb) {
-        mbar_wait(&tfull_bar[acc.stage], acc.phase, 4);
-        tc_fence_after_sync();
-        const uint32_t tacc = tmem_base + acc.stage * BN + (static_cast<uint32_t>(cx.quad * 32) << 16);
+        mbar_wait(afull_bar, acc_phase, 4);
         epi.tile(ep, ws, cx, tacc, nb);
-        tc_fence_before_sync();
         __syncwarp();
-        if (lane == 0) {
-          if (CG == 1 || leader) mbar_arrive(&tempty_bar[acc.stage]);
-          else mbar_arrive_cluster(&tempty_bar[acc.stage], 0);
-        }
-        acc.advance();
+        if (lane == 0) mbar_arrive(aempty_bar);
+        acc_phase ^= 1;
       }
       epi.end_work(ep, ws, cx);
     }
     epi.end_kernel(ep, cx);
   }
 
-  tc_fence_before_sync();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) tmem_dealloc<CG>(tmem_base, kTmemCols);
+  // no CTA of a pair may exit while its peer can still multicast into it or arrive on its barriers
+  if constexpr (CG == 2) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -276,7 +288,7 @@ cudaError_t launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const WorkSha
   if (clusters < 1) clusters = 1;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(clusters * CG);
-  cfg.blockDim = dim3(128 + 32 * EPI_WARPS);
+  cfg.blockDim = dim3(256 + 32 * EPI_WARPS);
   cfg.dynamicSmemBytes = Plan::kDynamicBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];

@@ -1,4 +1,4 @@
-// gemm_store.cuh — "store" epilogue of the tcgen05 GEMM: bias, erf-GELU (two closed forms, see gelu_erf2 / gelu_logistic2), residual add, bf16
+// gemm_store.cuh — "store" epilogue of the wgmma GEMM: bias, erf-GELU (two closed forms, see gelu_erf2 / gelu_logistic2), residual add, bf16
 // output through shared memory + TMA store (or fp32 output by direct stores).  Covers the encoder's
 // linear layers K2/K4/K5/K6/K7 of SURVEY.md §2.3 (HF RobertaSelfAttention / RobertaSelfOutput /
 // RobertaIntermediate / RobertaOutput reached from model/models.py:150-151, and embeddingHead,
@@ -25,8 +25,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return r;
 }
 
-// Packed fp32 pairs (Blackwell FFMA2 / fma.rn.f32x2): the FP32 pipe, not the issue rate, bounds the GELU
-// epilogue, and FFMA2 does two elements per slot at full fp32 precision.
+// fp32 pairs held in one 64-bit value: the GELU forms below are written pairwise; each op is the correctly rounded
+// scalar fp32 op on both halves.
 __device__ __forceinline__ uint64_t pack2(float a, float b) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
@@ -36,14 +36,14 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& a, float& b) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1), unpack2(b, b0, b1), unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1), unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
 // HF "gelu" = x * 0.5 * (1 + erf(x / sqrt(2))) = relu(x) - 0.5 |x| erfc(|x| / sqrt(2)), with
@@ -51,7 +51,7 @@ __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
 // and the 1/sqrt(2) folded into the coefficients.  Measured |error| of the GELU <= 7.1e-7 absolute (three
 // orders of magnitude below the bf16 rounding of the output).  The epilogue of the FFN-up GEMM is bound by
 // the SFU (MUFU) rate, so this form uses ONE MUFU (rcp) per element and no exponential; everything else is
-// packed FFMA2/FMUL2: per PAIR of elements 14 packed fp32 ops + 2 LOP + 2 MUFU.RCP.
+// FFMA/FMUL: per PAIR of elements 28 fp32 ops + 2 LOP + 2 MUFU.RCP.
 __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
   const uint64_t x = pack2(x0, x1);
   const uint64_t ax = x & 0x7FFFFFFF7FFFFFFFull;
@@ -75,7 +75,7 @@ __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
 // The same function in logistic form:  gelu(x) = x * Phi(x) = x / (1 + exp(-g(x))),  g = logit(Phi) fitted by an odd
 // degree-9 polynomial (minimax on the GELU itself over |x| <= 8; the leading coefficient is positive, so g -> +-inf
 // and the form saturates correctly for any |x|).  |error| <= 3.7e-6 absolute in fp32 (bf16 rounds the result at 2^-9
-// relative).  Per PAIR: 8 packed fp32 ops + 2 MUFU.EX2 + 2 MUFU.RCP  (gelu_erf2: 14 packed + 2 LOP + 2 MUFU.RCP).
+// relative).  Per PAIR: 16 fp32 ops + 2 MUFU.EX2 + 2 MUFU.RCP  (gelu_erf2: 28 fp32 ops + 2 LOP + 2 MUFU.RCP).
 __device__ __forceinline__ void gelu_logistic2(float& x0, float& x1) {
   const uint64_t x = pack2(x0, x1);
   const uint64_t t = mul2(x, x);
@@ -202,13 +202,12 @@ struct EpStore {
         tc05::mbar_arrive_expect_tx(rbar, kSlabBytes);
         tc05::tma_load_2d(slab, &p.tmR, rbar, col0, cx.row0, tc05::kEvictFirst);
       }
-      // 8 epilogue warps (168 registers each): both 32-column halves of the slab are requested from TMEM before the
-      // first is consumed.  16 warps (102 registers each): one half at a time.
+      // Up to 8 epilogue warps: both 32-column halves of the slab are read from the accumulator tile before the first
+      // is consumed.  16 warps (fewer registers each): one half at a time.
       constexpr bool kLean = EPI_WARPS > 8;
       uint32_t va[32], vb[kLean ? 1 : 32];
-      tc05::tmem_ld_32x32b_x32(tacc + col_in_tile, va);
-      if constexpr (!kLean) tc05::tmem_ld_32x32b_x32(tacc + col_in_tile + 32, vb);
-      tc05::tmem_ld_wait();
+      tc05::acc_ld_x32(tacc + col_in_tile, va);
+      if constexpr (!kLean) tc05::acc_ld_x32(tacc + col_in_tile + 32, vb);
       if (!tma_res && p.C) {
         // the slab is free once the previous TMA store has finished reading it
         if (issuer) tc05::bulk_wait_read_all();
@@ -219,8 +218,7 @@ struct EpStore {
         float f[32];
         if constexpr (kLean) {
           if (h == 1) {
-            tc05::tmem_ld_32x32b_x32(tacc + col_in_tile + 32, va);
-            tc05::tmem_ld_wait();
+            tc05::acc_ld_x32(tacc + col_in_tile + 32, va);
           }
 #pragma unroll
           for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(va[i]);

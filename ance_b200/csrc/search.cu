@@ -1,12 +1,12 @@
-// search.cu — flat inner-product top-k search on sm_100a.
+// search.cu — flat inner-product top-k search on sm_90a.
 //
 // Replaces faiss.IndexFlatIP(dim).add / .search as called by the reference at
 //   drivers/run_ann_data_gen.py:269-276,303 and drivers/run_ann_data_gen_dpr.py:238-252.
 //
 // Pipeline of one ance_index_search (all on the caller's stream):
 //   1. quantize_rows_kernel : Q fp32 -> 16-bit operands (+ ||q^||, ||q - q^|| per query)
-//   2. tc05_gemm_kernel<EpTopK> : coarse scores Q^ * P^^T on the tensor cores (tcgen05, TMEM
-//      accumulators); the epilogue never stores scores — every thread owns one query row, filters
+//   2. tc05_gemm_kernel<EpTopK> : coarse scores Q^ * P^^T on the tensor cores (wgmma, accumulator tile
+//      in shared memory); the epilogue never stores scores — every thread owns one query row, filters
 //      the 128 x BN tile against that query's running threshold and appends survivors to a
 //      per-query reservoir that a warp-cooperative radix select compacts to the best k'.
 //   3. rescore_kernel : exact scores (fp32 inputs, fp64 accumulate, one rounding to fp32) of the
@@ -164,8 +164,8 @@ template <int BN, int CAP>
 struct EpTopK {
   static constexpr uint64_t kHintA = tc05::kEvictLast;   // query tile: re-read for every corpus tile
   static constexpr uint64_t kHintB = tc05::kEvictNormal;  // corpus rows: every concurrently sweeping CTA pair re-reads
-                                                          // the same tile from L2 (EVICT_FIRST made each pair go to
-                                                          // HBM: 788 GB of DRAM reads for 13.6 GB of operands, ncu r01)
+                                                          // the same tile from L2 (EVICT_FIRST would make each pair
+                                                          // stream the whole operand from HBM by itself)
   static constexpr int kSlots = CAP / 32;
   static constexpr int kSmemBytes = 0;
   struct Params {
@@ -253,8 +253,7 @@ struct EpTopK {
 #pragma unroll 1
     for (int c = 0; c < BN; c += 32) {
       uint32_t v[32];
-      tmem_ld_32x32b_x32(tacc + c, v);
-      tmem_ld_wait();
+      acc_ld_x32(tacc + c, v);
       float m = __uint_as_float(v[0]);
 #pragma unroll
       for (int i = 1; i < 32; ++i) m = fmaxf(m, __uint_as_float(v[i]));
@@ -736,10 +735,11 @@ int check_device() {
     ance::set_error("no CUDA device: %s (libance_b200 has no CPU fallback)", cudaGetErrorString(e));
     return ANCE_ERR_CUDA;
   }
-  int major = 0;
+  int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) {
-    ance::set_error("device %d has compute capability %d.x; libance_b200 is built for sm_100a only", dev, major);
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) {
+    ance::set_error("device %d has compute capability %d.%d; libance_b200 is built for sm_90a only", dev, major, minor);
     return ANCE_ERR_CUDA;
   }
   return ANCE_OK;
@@ -786,8 +786,7 @@ int launch_coarse(ance_index* ix, const uint16_t* Q16, int64_t nq, int kprime, i
   if ((rc = ensure(&ix->cand_id, &ix->cand_ids, slots * out_cap))) return rc;
   // Soft barrier between the sweeping CTA pairs (gemm_core.cuh): pairs that sweep the SAME corpus rows share each tile
   // through L2 as long as they stay within `pace_window` tiles of each other.  Without it they drift apart and every one of
-  // them streams the rows from HBM by itself (ncu, round 1: 788 GB of DRAM reads for a 13.6 GB operand; measured round 2 at
-  // 18,944 and 75,776 queries: 910 -> 1213 TFLOP/s with the barrier).  Two shapes qualify: every item sweeps the whole
+  // them streams the rows from HBM by itself.  Two shapes qualify: every item sweeps the whole
   // corpus (n_splits == 1: all pairs pace each other), or one wave of (query tile, row range) items (pairs with the same
   // range pace each other).
   const int total_items = ws.num_m_blks * ws.n_splits;
@@ -896,8 +895,8 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
   int ns = 0;
   const bool bf = ix->fmt == ANCE_FMT_BF16;
 #define ANCE_COARSE(CG_, CAP_)                                                                                              \
-  rc = bf ? launch_coarse<256, (CG_ == 1 ? 4 : 6), CG_, CAP_, tc05::kFmtBF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st) \
-          : launch_coarse<256, (CG_ == 1 ? 4 : 6), CG_, CAP_, tc05::kFmtF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st)
+  rc = bf ? launch_coarse<128, 4, CG_, CAP_, tc05::kFmtBF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st) \
+          : launch_coarse<128, 4, CG_, CAP_, tc05::kFmtF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st)
   if (cg == 1 && cap == 1024) { ANCE_COARSE(1, 1024); }
   else if (cg == 1) { ANCE_COARSE(1, 2048); }
   else if (cap == 1024) { ANCE_COARSE(2, 1024); }
@@ -920,7 +919,7 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
   rp.pstats = ix->pstats;
   rp.mu = ix->centred ? ix->mu : nullptr;
   // Accumulation error of the coarse score c = fl(sum_i q^_i p^_i) on the tensor core.  The 16-bit x 16-bit products
-  // are exact in fp32; what is unspecified is how tcgen05.mma adds them (PTX: "precision at least that of fp32", order
+  // are exact in fp32; what is unspecified is how wgmma adds them (PTX: "precision at least that of fp32", order
   // and rounding implementation-defined; published measurements of earlier generations: truncation, block adds of
   // K = 16 aligned to the largest exponent).  Any such scheme performs at most d + d/16 additions, each with an error
   // of at most one ulp of the largest partial sum, 2^-23 * sum_i |q^_i p^_i| <= 2^-23 ||q^|| ||p^|| (Cauchy-Schwarz):

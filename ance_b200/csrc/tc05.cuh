@@ -1,9 +1,9 @@
-// tc05.cuh — sm_100a device primitives used by every tensor-core kernel in this repo:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st) and the
-// UMMA shared-memory / instruction descriptors.  Inline PTX only; no CUTLASS dependency.
+// tc05.cuh — sm_90a device primitives used by every tensor-core kernel in this repo:
+// mbarrier, TMA (cp.async.bulk.tensor, with cluster multicast), wgmma (warpgroup MMA with
+// shared-memory operand descriptors) and the shared-memory accumulator tiles the epilogues read.
+// Inline PTX only; no CUTLASS dependency.
 //
-// Bit layouts of the descriptors follow the PTX ISA "tcgen05 matrix descriptors" tables
-// (cross-checked against cute/arch/mma_sm100_desc.hpp of the vendored CUTLASS headers).
+// Bit layouts of the descriptors follow the PTX ISA "wgmma matrix descriptor" tables.
 #pragma once
 
 #include <cuda.h>
@@ -66,8 +66,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  // plain (CTA-scope release) form: the .release.cluster form costs a MEMBAR + ERRBAR per arrive
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
 __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity) {
@@ -85,22 +84,18 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
 }
 
 // Every wait in this repo goes through here.  A pipeline bug would otherwise hang the GPU; the
-// watchdog turns it into a trap (cudaErrorLaunchFailure on the host) after ~4 s of spinning.
+// watchdog turns it into a trap (cudaErrorLaunchFailure on the host) after ~4 s of spinning.  The trap
+// is inline: a function call here would make ptxas serialise every wgmma of the calling kernel.
 #ifndef TC05_WATCHDOG_CYCLES
 #define TC05_WATCHDOG_CYCLES 8000000000ll
 #endif
-static __device__ __noinline__ void mbar_timeout(uint32_t bar_addr, uint32_t parity, int tag) {
-  printf("[tc05] mbarrier timeout: block %d thread %d bar@0x%x parity %u tag %d\n", (int)blockIdx.x,
-         (int)threadIdx.x, bar_addr, parity, tag);
-  __trap();
-}
-
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+  (void)tag;   // call-site id: not reported, since printing it needs a call (above); each call site has its own trap
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3FFu) == 0 && clock64() - t0 > TC05_WATCHDOG_CYCLES) mbar_timeout(smem_u32(bar), parity, tag);
+    if ((++spins & 0x3FFu) == 0 && clock64() - t0 > TC05_WATCHDOG_CYCLES) asm volatile("trap;");
   }
 }
 
@@ -123,17 +118,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "memory");
 }
 
-// Same, issued by either CTA of a cta_group::2 pair: bytes complete on the LEADER CTA's barrier
-// (peer bit of the shared::cluster barrier address cleared).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0,
-                                                int c1, uint64_t hint) {
-  uint32_t bar_addr = smem_u32(bar) & 0xFEFFFFFFu;
+// Same, written to the same smem offset of every CTA of the cluster named by `cta_mask`; the bytes
+// complete on the barrier at the same offset in each of those CTAs.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0,
+                                                      int c1, uint16_t cta_mask, uint64_t hint) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
       :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar_addr), "r"(c0), "r"(c1),
-        "l"(hint)
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "h"(cta_mask), "l"(hint)
       : "memory");
 }
 
@@ -154,54 +148,20 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
-// ----------------------------------------------------------------------------------------------
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  }
-}
-
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05: descriptors
+// wgmma: descriptors
 // ----------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes
 // (64 x 16-bit) with the 128-byte swizzle (what a TMA box {64, rows} with SWIZZLE_128B writes).
 //   bits [ 0,14) start address >> 4      bits [16,30) leading byte offset >> 4 (unused here: 1)
-//   bits [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024)   bits [46,48) version = 1
-//   bits [49,52) base offset = 0 (tile base is 1024-B aligned)      bits [61,64) layout = 2 (SW128)
+//   bits [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024)
+//   bits [49,52) base offset = 0 (tile base is 1024-B aligned)      bits [62,64) layout = 1 (SW128)
+// A K step of 16 elements inside the 128-byte span advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
@@ -215,147 +175,92 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
 enum : uint32_t { kFmtF16 = 0, kFmtBF16 = 1 };
 
-// Instruction descriptor, kind::f16, fp32 accumulate.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt  [10,13) B fmt  [15] A major (0 = K)  [16] B major
-//   [17,23) N >> 3         [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t m, uint32_t n, uint32_t fmt, uint32_t a_mn_major,
-                                                      uint32_t b_mn_major) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-         ((m >> 4) << 24);
+// ----------------------------------------------------------------------------------------------
+// wgmma: issue / commit / wait.  All 128 threads of a warpgroup execute these together.
+// Accumulator fragment of m64nN (f32): thread t of the warpgroup holds, for j in [0, N/8),
+//   d[4j + 0..1] = D[16 (t/32) + (t%32)/4    ][8j + 2 (t%4) + 0..1]
+//   d[4j + 2..3] = D[16 (t/32) + (t%32)/4 + 8][8j + 2 (t%4) + 0..1]
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// operand lists of m64nNk16 with fp32 accumulators: N/2 registers per thread
+#define TC05_R8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define TC05_R32 TC05_R8(0), TC05_R8(8), TC05_R8(16), TC05_R8(24)
+#define TC05_R64 TC05_R32, TC05_R8(32), TC05_R8(40), TC05_R8(48), TC05_R8(56)
+#define TC05_S32                                                                  \
+  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "        \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define TC05_S64                                                                  \
+  TC05_S32 ", "                                                                   \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+// NAME, PTX shape + types, accumulator registers, their operand strings / constraints, operand numbers of the inputs
+#define TC05_WGMMA(NAME, INSTR, NR, SLIST, RLIST, IA, IB, IP, IT)                                                     \
+  template <int kTransB>                                                                                              \
+  __device__ __forceinline__ void NAME(float (&d)[NR], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {        \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" IP ", 0;\n\t" INSTR " {" SLIST "}, %" IA ", %" IB           \
+                 ", p, 1, 1, 0, %" IT ";\n\t}"                                                                        \
+                 : RLIST                                                                                              \
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransB));                                            \
+  }
+TC05_WGMMA(wgmma_m64n128k16_bf16, "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", 64, TC05_S64, TC05_R64, "64", "65", "66", "67")
+TC05_WGMMA(wgmma_m64n128k16_f16, "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16", 64, TC05_S64, TC05_R64, "64", "65", "66", "67")
+TC05_WGMMA(wgmma_m64n64k16_bf16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16", 32, TC05_S32, TC05_R32, "32", "33", "34", "35")
+TC05_WGMMA(wgmma_m64n64k16_f16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16", 32, TC05_S32, TC05_R32, "32", "33", "34", "35")
+
+// D (+)= A[smem] * B[smem], m64 x N x k16; kTransB = 1: B is MN-major
+template <uint32_t FMT, int kTransB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (FMT == kFmtBF16) wgmma_m64n128k16_bf16<kTransB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n128k16_f16<kTransB>(d, adesc, bdesc, accumulate);
+}
+template <uint32_t FMT, int kTransB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (FMT == kFmtBF16) wgmma_m64n64k16_bf16<kTransB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n64k16_f16<kTransB>(d, adesc, bdesc, accumulate);
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: MMA issue / commit (single issuing thread)
+// accumulator tiles in shared memory: fp32, row-major, `pitch` words per row (pitch % 32 == 4: the
+// row-per-thread reads below are free of bank conflicts).  The wgmma fragment of rows [r0, r0 + 64) is
+// written by its warpgroup; afterwards any thread reads whole 32-column chunks of one row.
 // ----------------------------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}"
-        :
-        : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}"
-        :
-        : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+template <int R>
+__device__ __forceinline__ void acc_store_frag(float* tile, int pitch, int r0, int c0, const float (&d)[R]) {
+  const int t = threadIdx.x & 127;
+  const int r = r0 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c = c0 + 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(tile + r * pitch + c + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(tile + (r + 8) * pitch + c + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]   (A: lane = row, each 32-bit column = two consecutive K elements)
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        :
-        : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        :
-        : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
+// 32 consecutive fp32 accumulator words at shared-memory WORD address `waddr` (byte address / 4)
+__device__ __forceinline__ void acc_ld_x32(uint32_t waddr, uint32_t* v) {
+#pragma unroll
+  for (int i = 0; i < 32; i += 4)
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v[i]), "=r"(v[i + 1]), "=r"(v[i + 2]), "=r"(v[i + 3])
+                 : "r"((waddr + i) * 4u)
+                 : "memory");
 }
-
-// mbarrier arrive once all tcgen05 ops previously issued by this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// cta_group::2: arrive on the barrier at this smem offset in every CTA named by cta_mask
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers.  Warp w of a CTA may only touch lanes [32*(w%4), 32*(w%4)+32).
-// taddr = (lane << 16) | column
-// ----------------------------------------------------------------------------------------------
-// pointer form: `v` must point into a register-resident array indexed with compile-time constants
-__device__ __forceinline__ void tmem_ld_32x32b_x32p(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-        "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // ring-buffer bookkeeping

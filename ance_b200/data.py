@@ -6,7 +6,7 @@ Drop-in for the reference's
   * ``GetProcessingFn``    data/msmarco_data.py:275-303 and data/DPR_data.py:276-296
 with the same names, argument meaning and error behaviour, so the trainer (which random-accesses
 the same caches, data/msmarco_data.py:348-358) and any code written against the reference keep
-working.  ``StridedBatchReader`` is what the B200 refresher itself uses: it memory-maps the file
+working.  ``StridedBatchReader`` is what the GPU refresher itself uses: it memory-maps the file
 once, takes this rank's ``i % world_size == rank`` records with numpy (no per-record Python), and
 yields pinned ``(ids int32[B,L], lens int32[B], idx int64[B])`` batches; the attention mask is
 built on the GPU from ``lens`` (or from ``ids != 0`` for DPR).

@@ -1,4 +1,4 @@
-"""B200-native ANN refresher — drop-in for the reference's drivers/run_ann_data_gen.py.
+"""H100-native ANN refresher — drop-in for the reference's drivers/run_ann_data_gen.py.
 
 Same CLI flags, same inputs (`training_dir/checkpoint-N/` with scheduler.pt, `data_dir/{passages,
 train-query,dev-query}` token caches + qrels) and same outputs (`output_dir/ann_training_data_N`,
@@ -8,10 +8,10 @@ picks the files up at run_ann.py:182-228).  What changes is where the work happe
   reference (run_ann_data_gen.py)                       here
   ---------------------------------------------------   ------------------------------------------------
   per-record Python dataloader, batch 16 (199-202)      StridedBatchReader: memmap + numpy stride, pinned
-  HF eager fp32 forward, D2H every batch (175-180)      libance_b200 encoder (tcgen05 GEMMs, fused attention);
+  HF eager fp32 forward, D2H every batch (175-180)      libance_b200 encoder (wgmma GEMMs, fused attention);
                                                         embeddings stay in this rank's HBM
   np.save / np.load gather to rank 0 (util.py:87-146)   rows never move; ONE all-gather of query embeddings
-  faiss.IndexFlatIP on rank 0, 16 threads (269-303)     per-shard sm_100a flat-IP top-k + host k-way merge
+  faiss.IndexFlatIP on rank 0, 16 threads (269-303)     per-shard sm_90a flat-IP top-k + host k-way merge
   Python loops for negatives / NDCG (339-440)           numpy (ance_b200/postprocess.py)
 
 Row numbering is the reference's: rank r encodes records r, r+W, ...; global row = (rows of ranks
@@ -166,8 +166,8 @@ class B200Backend:
         B = args.per_gpu_eval_batch_size
         # super-batch = what one encoder pass holds.  Only the MaxP row layout depends on the reference's batch size
         # (chunk-major per `per_gpu_eval_batch_size` documents, run_ann_data_gen.py:183-186): there it must be a multiple
-        # of B; elsewhere B has no effect on the result and the pass is filled completely (592 x 128 tokens = whole waves
-        # of 256-row GEMM tiles on 148 SMs).
+        # of B; elsewhere B has no effect on the result and the pass is filled completely (592 x 128 tokens = 592 row
+        # tiles of the encoder GEMMs).
         per = max(B, (args.encode_batch_tokens // L) // B * B) if multi else max(1, args.encode_batch_tokens // L)
         bucketed = self.mask_mode != "nonzero" and not multi and getattr(args, "length_buckets", True)
         varlen = bucketed and L <= 128 and getattr(args, "varlen", True) and hasattr(self.model, "encode_lens_varlen")
@@ -261,9 +261,9 @@ def all_gather_ids(ids: np.ndarray, device) -> np.ndarray:
     return all_gather_rows(t[:, None])[:, 0].cpu().numpy()
 
 
-#: queries per search block: four full waves of the coarse kernel on a B200 (74 CTA pairs x 256 query rows each).  One wave
-#: per block (18,944) left ~28 ms of per-call latency (stream sync for the tier counters, all-to-all, staging) for every
-#: 32 ms of kernels when the corpus is spread over 8 GPUs; the merge of a block still overlaps the next block's search.
+#: queries per search block: 296 query tiles of 256 rows.  Large blocks amortise the per-call latency (stream sync for the
+#: tier counters, all-to-all, staging) when the corpus is spread over several GPUs; the merge of a block still overlaps the
+#: next block's search.
 QUERY_BLOCK = 75776
 
 
@@ -547,7 +547,7 @@ def generate_new_ann(args, output_num, checkpoint_path, training_query_positive_
 
 
 # =============================================================================================
-# CLI (flags of run_ann_data_gen.py:443-627, plus three B200 knobs at the end)
+# CLI (flags of run_ann_data_gen.py:443-627, plus three GPU knobs at the end)
 # =============================================================================================
 def get_arguments(argv=None):
     p = argparse.ArgumentParser()
@@ -576,7 +576,7 @@ def get_arguments(argv=None):
     p.add_argument("--inference", default=False, action="store_true")
     p.add_argument("--config_name", default="", type=str)
     p.add_argument("--tokenizer_name", default="", type=str)
-    # B200 knobs (not in the reference)
+    # GPU knobs (not in the reference)
     p.add_argument("--search_operand", default="auto", choices=["auto", "fp16", "bf16"],
                    help="16-bit operand format of the coarse tensor-core pass (results are exact either way); auto = fp16, "
                         "falling back to bf16 when a row or a query leaves the fp16 range")
@@ -603,7 +603,7 @@ def set_env(args):
     if args.local_rank == -1 and "LOCAL_RANK" in os.environ and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         args.local_rank = int(os.environ["LOCAL_RANK"])
     if args.no_cuda or not torch.cuda.is_available():
-        raise RuntimeError("ance_b200 has no CPU fallback: the refresher needs an sm_100 GPU (drop --no_cuda)")
+        raise RuntimeError("ance_b200 has no CPU fallback: the refresher needs an sm_90 GPU (drop --no_cuda)")
     if args.local_rank == -1:
         args.device = torch.device("cuda", torch.cuda.current_device())
         args.n_gpu = 1

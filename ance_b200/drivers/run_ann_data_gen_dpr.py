@@ -1,4 +1,4 @@
-"""B200-native ANN refresher for DPR / OpenQA — drop-in for the reference's drivers/run_ann_data_gen_dpr.py
+"""H100-native ANN refresher for DPR / OpenQA — drop-in for the reference's drivers/run_ann_data_gen_dpr.py
 (BASELINE config 5: 21M Wikipedia passages, BERT-base bi-encoder, top-100).
 
 Same flags, inputs and outputs as the reference; encode and search run through libance_b200 exactly as in
@@ -197,7 +197,7 @@ def get_arguments(argv=None):
     p.add_argument("--passage_path", default=None, type=str, required=True)
     p.add_argument("--test_qa_path", default=None, type=str, required=True)
     p.add_argument("--trivia_test_qa_path", default=None, type=str, required=True)
-    # B200 knobs
+    # GPU knobs
     p.add_argument("--search_operand", default="auto", choices=["auto", "fp16", "bf16"])
     p.add_argument("--encode_batch_tokens", default=75776, type=int)
     p.add_argument("--seed", default=None, type=int)

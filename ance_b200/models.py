@@ -1,4 +1,4 @@
-"""``--model_type`` plugin registry and the dual-encoder classes, B200-native.
+"""``--model_type`` plugin registry and the dual-encoder classes, H100-native.
 
 Mirrors the reference's plugin surface (model/models.py:289-322):
 
@@ -9,7 +9,7 @@ Mirrors the reference's plugin surface (model/models.py:289-322):
 
 The classes are ``nn.Module``s whose parameters carry the checkpoint's own key names (SURVEY.md §8 a2),
 so ``load_state_dict`` / ``.to(device)`` / DDP wrapping behave as with the reference; the forward
-is NOT PyTorch: ``query_emb`` / ``body_emb`` run the hand-written sm_100a encoder of
+is NOT PyTorch: ``query_emb`` / ``body_emb`` run the hand-written sm_90a encoder of
 libance_b200.so (csrc/encoder.cu).  There is no CPU path — calling them with CPU tensors raises.
 The training ``forward()`` losses (models.py:58-134,260-271) are out of scope for this package.
 """
@@ -209,8 +209,8 @@ _CudaEncoder.forward_varlen = _forward_varlen
 class _B200Encoder(nn.Module):
     """Common machinery: lazily (re)build the CUDA encoder when the parameters move or change."""
 
-    #: tokens processed per launch sequence (activations: ~14 KB per token).  75,776 = 296 row blocks of 256:
-    #: every encoder GEMM then has a tile count divisible by the 74 CTA pairs of a B200 (no partial last wave).
+    #: tokens processed per launch sequence (activations: ~14 KB per token).  75,776 = 592 row blocks of 128 (the GEMM's
+    #: row tile); about 1 GB of activations.
     max_tokens = int(os.environ.get("ANCE_B200_MAX_TOKENS", 75776))
 
     #: 16-bit storage format of weights and activations inside the CUDA encoder: "fp16" (11 significant bits; the
@@ -221,7 +221,7 @@ class _B200Encoder(nn.Module):
 
     def _enc_for(self, name, backbone, arch, heads, pad_id, head, device) -> _CudaEncoder:
         if device.type != "cuda":
-            raise _lib.AnceError("ance_b200 models run on an sm_100 GPU only (no CPU fallback): move the model and "
+            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback): move the model and "
                                  "the inputs to a CUDA device")
         cache = self.__dict__.setdefault("_enc_cache", {})
         # Rebuild the device copy when a parameter was written in place (load_state_dict / optimizer step bump
@@ -248,7 +248,7 @@ class _B200Encoder(nn.Module):
     @staticmethod
     def _prep(input_ids, attention_mask):
         if input_ids.device.type != "cuda":
-            raise _lib.AnceError("ance_b200 models run on an sm_100 GPU only (no CPU fallback)")
+            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
         ids = input_ids.to(torch.int32).contiguous()
         mask = (attention_mask != 0).to(torch.uint8).contiguous()
         return ids, mask
@@ -343,7 +343,7 @@ class RobertaDot_NLL_LN(_B200Encoder):
     def body_emb(self, input_ids, attention_mask):
         return self.query_emb(input_ids, attention_mask)
 
-    # fast path used by the B200 refresher: mask given as lengths (msmarco_data.py:282 form)
+    # fast path used by the GPU refresher: mask given as lengths (msmarco_data.py:282 form)
     def encode_lens(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         return self._encoder(ids_i32.device).forward(ids_i32.contiguous(), lens_i32.contiguous(), None, out=out)
 
@@ -484,7 +484,7 @@ def _reference_seed_class():
         return ref_cls
     except Exception as e:  # ImportError, or the reference's own third-party imports failing
         raise NotImplementedError(
-            "seeddot_nll (SEED-Encoder, model/models.py:201-221) has no sm_100a kernels in ance_b200 — its backbone is a "
+            "seeddot_nll (SEED-Encoder, model/models.py:201-221) has no sm_90a kernels in ance_b200 — its backbone is a "
             "vendored fairseq-style model outside the ANN-refresh scope (SURVEY.md par. 2.1 row 8) — and the reference's "
             "stock module could not be imported to fall back to ({}: {}).  Put the reference checkout on sys.path to run "
             "seeddot_nll through its own PyTorch code.".format(type(e).__name__, e)) from e
@@ -493,7 +493,7 @@ def _reference_seed_class():
 class SEEDEncoderDot_NLL_LN:
     """model/models.py:201-221 (`seeddot_nll`).  The registry name resolves; construction / from_pretrained FALL BACK to
     the reference's stock PyTorch module (SURVEY.md par. 2.1 row 8): the object returned is the reference's class, so
-    `query_emb` / `body_emb` behave exactly as upstream (no B200 acceleration)."""
+    `query_emb` / `body_emb` behave exactly as upstream (no GPU acceleration)."""
 
     def __new__(cls, *a, **k):
         return _reference_seed_class()(*a, **k)

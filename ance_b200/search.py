@@ -1,4 +1,4 @@
-"""faiss.IndexFlatIP-shaped front end of the sm_100a flat inner-product search.
+"""faiss.IndexFlatIP-shaped front end of the sm_90a flat inner-product search.
 
 Mirrors the three calls the reference makes (drivers/run_ann_data_gen.py:269-276,303):
 
@@ -9,7 +9,7 @@ Mirrors the three calls the reference makes (drivers/run_ann_data_gen.py:269-276
 copy).  The multi-GPU form of SURVEY.md §8(e) — rows stay on the rank that encoded them, queries are
 all-gathered once, per-shard top-k lists are merged on the host with ``merge_topk_host`` — lives in
 ``ance_b200.drivers.run_ann_data_gen.sharded_search``.
-There is no CPU fallback: without libance_b200.so and an sm_100 GPU every call raises.
+There is no CPU fallback: without libance_b200.so and an sm_90 GPU every call raises.
 """
 from __future__ import annotations
 
@@ -50,7 +50,7 @@ class IndexFlatIP:
         storage: a CUDA fp32 tensor [capacity, d] to use as the index's row storage (kept alive by the index).  Rows
         written into `storage[i:i+n]` by their producer and then passed to add() are added without a copy."""
         if not torch.cuda.is_available():
-            raise _lib.AnceError("ance_b200.IndexFlatIP needs a CUDA device (sm_100); there is no CPU fallback")
+            raise _lib.AnceError("ance_b200.IndexFlatIP needs a CUDA device (sm_90); there is no CPU fallback")
         self._lib = _lib.load()
         self.d = int(d)
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())

@@ -13,12 +13,14 @@ value = (passages encoded + queries searched) per second, whole job; `stages` gi
 Workloads (--workload; the default is the one BASELINE.json's metric is quoted on):
   marco_psg        BASELINE configs[1]: rdot_nll RoBERTa-base, passages L=128, queries L=64, 8,841,823 x 768 index, top-200
   marco_doc_maxp   configs[3]: rdot_nll_multi_chunk, documents 2048 = 4 x 512 chunks, 12,855,340 x 768 chunk-row index, top-200
-  dpr              configs[4]: DPR BiEncoder (BERT-base, CLS, no head), L=256, 21,015,324 x 768 un-normalised rows, top-100
+  dpr              configs[4]: DPR BiEncoder (BERT-base, CLS, no head), L=256, 10,507,662 x 768 un-normalised rows (half of
+                   the 21M corpus, so that one 80 GB H100 holds the index), top-100
 
   python bench.py --gpus 1 --steps 5 --warmup 3
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
   python bench.py --impl reference ...     # the reference's CPU arithmetic on the host cores (see run_reference)
+  python bench.py ... --dump-outputs DIR   # also write what the last timed step computed as DIR/*.npy
 """
 from __future__ import annotations
 
@@ -50,9 +52,10 @@ WORKLOADS = {
         unit="documents+queries/s", model="rdot_nll_multi_chunk", L_p=2048, L_q=64, chunks=4, n_index=12855340, topk=200,
         pb=2368, qb=296, index_kind="layernorm_clustered", head=True),
     "dpr": dict(
-        title="BASELINE configs[4]: DPR 21M Wikipedia passages, BiEncoder (BERT-base CLS) seq_len=256, encode + top-100",
-        metric="ANN-refresh throughput: passages encoded/sec + queries top-100/sec, 21M x 768",
-        unit="passages+queries/s", model="dpr", L_p=256, L_q=256, chunks=1, n_index=21015324, topk=100,
+        title="BASELINE configs[4]: DPR Wikipedia passages, BiEncoder (BERT-base CLS) seq_len=256, encode + top-100 over "
+              "10,507,662 rows (half of the 21M corpus: fp32 rows + 16-bit operands of all 21M take 97 GB, one H100 has 80)",
+        metric="ANN-refresh throughput: passages encoded/sec + queries top-100/sec, 10.5M x 768",
+        unit="passages+queries/s", model="dpr", L_p=256, L_q=256, chunks=1, n_index=10507662, topk=100,
         pb=18944, qb=296, index_kind="dpr", head=False),
 }
 
@@ -77,7 +80,7 @@ def peaks():
         j = json.load(open(p))
         return {"bf16_tflops": j.get("bf16_tflops_sustained", j.get("bf16_tflops")), "hbm_gbs": j.get("hbm_gbs"),
                 "source": "MEASURED_PEAKS.json (bf16_tflops_sustained: the kernel is timed inside a long step)"}
-    return {"bf16_tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md, sustained)"}
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "fallback: H100 SXM data sheet, dense, 700 W (not measured)"}
 
 
 class ClockSampler(threading.Thread):
@@ -174,7 +177,7 @@ def cpu_search_topk(P: torch.Tensor, Q: torch.Tensor, k: int, threads: int, p_bl
 
 def _pick_threads(fn, thread_sets):
     """Time `fn` once per candidate thread count on a small probe and return the fastest (small fp32 GEMMs stop scaling —
-    and regress — far below the 128+ hardware threads of a B200 host, so "all cores" is not automatically the best the
+    and regress — far below the 100+ hardware threads of a GPU host, so "all cores" is not automatically the best the
     reference's CPU path can do; both it and the reference's own 16 (run_ann_data_gen.py:269) are tried)."""
     best_t, best_th = None, thread_sets[0]
     for th in thread_sets:
@@ -192,7 +195,7 @@ def _pick_threads(fn, thread_sets):
 def cpu_step_sample(wl, n_p, n_q, search_q, search_rows, want_outputs=False):
     """Time a bounded sample of one step on the CPU.  Returns rates (units/s; the search rate is scaled linearly in the
     row count to the workload's index size), what was used, and optionally the sample's inputs / outputs for the
-    parity block of the B200 arm."""
+    parity block of the GPU arm."""
     cores = os.cpu_count() or 1
     thread_sets = sorted({cores, min(cores, 64), min(cores, 16)}, reverse=True)
     orc = _cpu_models(wl)
@@ -330,7 +333,7 @@ def run_reference(args, wl):
 
 
 # =============================================================================================
-# B200 arm
+# GPU arm
 # =============================================================================================
 def build_model(wl, dev, encoder_operand):
     from ance_b200.models import BiEncoder, RobertaDot_CLF_ANN_NLL_MultiChunk, RobertaDot_NLL_LN
@@ -402,6 +405,7 @@ def run_b200(args, wl):
             model.encode_lens(ids, lens, out=step_rows)
 
     pending = []      # N > 1: the previous slice's search, issued but not yet merged / gathered
+    last = {}         # what the latest timed step handed back: query embeddings, merged top-k labels
 
     def step_value():
         step_index.reset()
@@ -409,10 +413,13 @@ def run_b200(args, wl):
         step_index.add(step_rows)          # in place: the rows were written into the index's own storage
         step_index.prepare()               # column mean + centred 16-bit operands + norm statistics of the added rows
         q = model.query_emb(q_ids_d, q_ids_d != 0) if mask_form else model.encode_lens(q_ids_d, q_len_d)
+        last["q"] = q
         if world == 1:
-            return sharded_search(local_search, n_local, q.contiguous(), k, row_offset=row_offset)   # numpy labels
+            last["labels"] = sharded_search(local_search, n_local, q.contiguous(), k, row_offset=row_offset)   # numpy labels
+            return last["labels"]
         q_all = torch.empty((qb * world, DIM), dtype=torch.float32, device=dev)
         dist.all_gather_into_tensor(q_all, q.contiguous())
+        last["q"] = q_all   # the merged labels are for these rows, every rank's queries
         # As in the driver's block loop, the host merge of this slice's lists overlaps the device work that follows: the
         # search is issued here and finished (merge waited for, labels gathered on rank 0) after the NEXT slice has been
         # enqueued; `drain()` finishes the last one inside the timed region.
@@ -421,7 +428,7 @@ def run_b200(args, wl):
 
     def drain():
         while pending:
-            pending.pop(0).finish()
+            last["labels"] = pending.pop(0).finish()   # rank 0: the merged labels of the slice; other ranks: None
 
     def step_e2e():
         """The calls a user of the reference makes (run_ann_data_gen.py:172-180,269-303), host buffers in, numpy out:
@@ -476,6 +483,8 @@ def run_b200(args, wl):
         sampler.start()
     ms = timed(step_value, args.steps, wall=False)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step_rows, last)
     prof = _lib.profile_read(reset=True)
     _lib.profile_enable(False)
     launches = _lib.load().ance_launch_count() - launches0
@@ -521,12 +530,6 @@ def run_b200(args, wl):
     enc_ms = gemm_ms + prof["attention"][0] + prof["norm_embed"][0]
     srch_ms = coarse_ms + prof["rescore"][0] + prof["exact"][0]     # + the queries' share of `quantize` (negligible)
     alg_flop = args.steps * (seqs_p * flop_seq(Lc, head) + qb * flop_seq(L_q, head))
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "r02_ncu_gemm_traffic.json")
-    if not os.path.exists(tp):
-        tp = os.path.join(ROOT, "profiles", "r01_ncu_gemm_traffic.json")
-    if os.path.exists(tp) and wl is WORKLOADS["marco_psg"]:
-        traffic = json.load(open(tp)).get("dram_bytes_per_launch")
     out = {
         "metric": wl["metric"], "value": units / ms * 1e3, "unit": wl["unit"], "n_gpus": world, "steps": args.steps,
         "warmup": warm, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
@@ -548,7 +551,7 @@ def run_b200(args, wl):
         },
         "roofline": {"kernel": "tc05_gemm_kernel<EpStore> (encoder linear layers)", "bound": "tensor",
                      "achieved": gemm_tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": gemm_tf / pk["bf16_tflops"],
-                     "traffic": traffic, "peak_source": pk["source"], "launches": gemm_n,
+                     "peak_source": pk["source"], "launches": gemm_n,
                      "avg_launch_ms": gemm_ms / max(gemm_n, 1),
                      "share_of_step": gemm_ms / (ms * args.steps)},
         "e2e": {"value": units / ms_e2e * 1e3, "unit": wl["unit"],
@@ -568,7 +571,7 @@ def run_b200(args, wl):
             "value": cpu_value(pb, qb, info), "unit": wl["unit"], "cores": max(info["encode_threads"], info["search_threads"]),
             "kind": "port", "sample": sample_text(wl, base_sample, info) + "; %.0f s of CPU work" % info["seconds"],
             "passages_per_s": info["rate_p"], "queries_topk_per_s": info["qps_full"], "search_kind": info["search_kind"]}
-        # parity of the B200 path with the CPU arm on the very sample the CPU arm just computed (checker use of oracle/)
+        # parity of the GPU path with the CPU arm on the very sample the CPU arm just computed (checker use of oracle/)
         with torch.no_grad():
             pi = o["p_ids"].to(dev)
             if wl["model"] == "dpr":
@@ -592,15 +595,43 @@ def run_b200(args, wl):
             "search_topk_lists_identical_frac_vs_cpu_fp32": same, "search_topk_set_overlap_vs_cpu_fp32": setov,
             "search_score_max_rel_diff": float(((torch.from_numpy(Dg) - o["D"]).abs().max() / o["D"].abs().max())),
             "note": "CPU fp32 sgemm sums in a different order than the canonical fp64-accumulated score: lists may differ "
-                    "only where two scores are closer than fp32 summation noise; bit-exact parity vs the oracle is in tests/",
-            "overlap_at_200_vs_fp32_encoded_corpus": _load_overlap()}
+                    "only where two scores are closer than fp32 summation noise; bit-exact parity vs the oracle is in tests/"}
     print(json.dumps(out))
 
 
-def _load_overlap():
-    """The 20,480-passage overlap@200 gate is a GPU test (tests/test_gpu_encoder.py); its last committed result."""
-    p = os.path.join(ROOT, "profiles", "r02_overlap_at_200.json")
-    return json.load(open(p)) if os.path.exists(p) else None
+DUMP_PASSAGE_ROWS = 12288   # seeded sample of the step's passage embeddings (37888 x 768 fp32 would be 116 MB)
+DUMP_QUERY_ROWS = 2048      # seeded sample of the searched queries (embeddings + their top-k labels)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, step_rows, last):
+    """What the last timed step computed, as a caller of that path receives it: the passage embeddings written into the
+    index, the query embeddings and the merged top-k labels of those queries (int64 row ids, stored as float64, exact below
+    2^53).  Passages and queries are fixed, seeded samples of rows (their row numbers are written beside them), so the
+    files stay under 64 MB whatever the step size or the number of GPUs.  The inputs are seeded, so two builds given the
+    same arguments can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+
+    def sample(n, cap, seed):
+        return np.sort(np.random.default_rng(seed).choice(n, size=min(n, cap), replace=False))
+
+    p_sel = sample(step_rows.shape[0], DUMP_PASSAGE_ROWS, 0)
+    q = last["q"]
+    q_sel = sample(q.shape[0], DUMP_QUERY_ROWS, 1)
+    arrays = {
+        "passage_rows": p_sel.astype(np.float64),
+        "passage_embeddings": step_rows[torch.from_numpy(p_sel).to(step_rows.device)].float().cpu().numpy(),
+        "query_rows": q_sel.astype(np.float64),
+        "query_embeddings": q[torch.from_numpy(q_sel).to(q.device)].float().cpu().numpy(),
+    }
+    if last.get("labels") is not None:
+        labels = np.asarray(last["labels"])
+        assert labels.shape[0] == q.shape[0], (labels.shape, q.shape)
+        arrays["topk_labels"] = labels[q_sel].astype(np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_MAX_BYTES, f"--dump-outputs would write {total} bytes (limit {DUMP_MAX_BYTES})"
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -615,6 +646,8 @@ def main():
     ap.add_argument("--search_operand", default="auto", choices=["auto", "fp16", "bf16"])
     ap.add_argument("--encoder_operand", default="fp16", choices=["fp16", "bf16"])
     ap.add_argument("--no_cpu_baseline", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     # defaults: marco_psg 64 encoder passes of 592 x 128 tokens + 2 of 1184 x 64 (16:1, the refresh's own 17.6:1);

@@ -1,4 +1,4 @@
-/* ance_b200.h — C ABI of libance_b200.so: the B200-native replacement for the native arithmetic on
+/* ance_b200.h — C ABI of libance_b200.so: the H100-native replacement for the native arithmetic on
  * microsoft/ANCE's ANN-refresh path (drivers/run_ann_data_gen.py + model/models.py).
  *
  * The reference has no FFI of its own: the native work on this path is done by un-vendored
@@ -8,7 +8,7 @@
  * on the device that was current when the handle was created; `stream` is a cudaStream_t passed as
  * void*.  Handles are not thread-safe; distinct handles may be used concurrently.
  *
- * There is NO CPU fallback: every compute entry point fails with ANCE_ERR_CUDA when no sm_100
+ * There is NO CPU fallback: every compute entry point fails with ANCE_ERR_CUDA when no sm_90
  * device is present.
  */
 #ifndef ANCE_B200_H_
@@ -23,12 +23,12 @@ extern "C" {
 enum {
   ANCE_OK = 0,
   ANCE_ERR_INVALID = 1,     /* bad argument */
-  ANCE_ERR_CUDA = 2,        /* CUDA runtime / driver error, or no sm_100 device */
+  ANCE_ERR_CUDA = 2,        /* CUDA runtime / driver error, or no sm_90 device */
   ANCE_ERR_NOMEM = 3,
   ANCE_ERR_UNSUPPORTED = 4  /* shape outside what the kernels were built for */
 };
 
-/* 16-bit operand format of the tensor-core passes (tcgen05 kind::f16 runs both at the same rate). */
+/* 16-bit operand format of the tensor-core passes (wgmma runs both at the same rate). */
 enum { ANCE_FMT_FP16 = 0, ANCE_FMT_BF16 = 1 };
 
 const char* ance_version(void);
@@ -166,7 +166,7 @@ int ance_encoder_forward_varlen(ance_encoder_t enc, const int32_t* ids_dev, cons
 /* Tunables: "prune_last_layer" (default 1): in the last layer only token 0 of every sequence is read
  * downstream, so out-projection / FFN / LayerNorm run on those rows only (result-identical; bench.py reports
  * the executed FLOPs beside the algorithmic ones).  "ln_rows_per_warp" (1, 2, 4, or 3 = two rows held packed; default 2, process-wide): rows a warp
- * of the LayerNorm kernel normalises side by side (bit-identical results; 2 is the fastest on B200).  "varlen_align" (1 | 16):
+ * of the LayerNorm kernel normalises side by side (bit-identical results; default 2).  "varlen_align" (1 | 16):
  * see ance_encoder_forward_varlen. */
 int ance_encoder_set_param(ance_encoder_t enc, const char* name, double value);
 /* Input / output validation, deferred so that forward stays asynchronous: synchronises `stream` and returns

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real sm_100 GPU (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a real sm_90 GPU (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

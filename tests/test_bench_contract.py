@@ -1,5 +1,5 @@
 """The CPU arm of bench.py (`--impl reference`) prints the contract's JSON line: checked here with a tiny sample
-(ANCE_BENCH_TINY_CPU) so that the CPU suite stays fast; the GPU arm is exercised by the driver on a B200."""
+(ANCE_BENCH_TINY_CPU) so that the CPU suite stays fast; the GPU arm is exercised by the driver on an H100."""
 import json
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a encoder with (i) the golden outputs of the reference's own classes
+"""Parity of the sm_90a encoder with (i) the golden outputs of the reference's own classes
 (tests/golden/encoder_*.npz, fp32 HF eager) and (ii) the CPU oracle layer by layer.
 
 Tolerance (floating point, stated once; BASELINE.md par. 5): weights and activations are stored in fp16
@@ -225,7 +225,7 @@ def test_fp16_overflow_is_reported_not_silent():
 
 
 def test_retrieval_overlap_at_200(rdot):
-    """BASELINE.md par. 5's second encoder gate: encode a 20,480-passage / 512-query 12-layer fixture with the sm_100a
+    """BASELINE.md par. 5's second encoder gate: encode a 20,480-passage / 512-query 12-layer fixture with the sm_90a
     encoder and with the fp32 oracle, run the ORACLE search (exact fp32 inner product, top-200) on both embedding sets
     and compare the neighbour sets the trainer would consume.  The fp32 side is oracle.encoder_oracle placed on the GPU
     (plain fp32, TF32 off) and tied to its CPU run on a slice."""

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a flat inner-product search with the CPU oracle (bit-exact: int64 labels and
+"""Parity of the sm_90a flat inner-product search with the CPU oracle (bit-exact: int64 labels and
 fp32 scores), through the C ABI (ance_b200.search.IndexFlatIP -> ctypes -> libance_b200.so)."""
 import os
 
@@ -236,7 +236,7 @@ def test_tier2_threshold_pass_is_cheap_and_exact():
 
 def test_tensor_core_accumulation_error_is_inside_the_certificate_bound(lib):
     """The certificate charges d * 2^-22 * |q^| |p^| for the tensor core's fp32 accumulation (search.cu,
-    coarse_rescore_pass).  Measure the real thing: tcgen05 scores of 16-bit operands against the fp64 dot product of
+    coarse_rescore_pass).  Measure the real thing: tensor-core scores of 16-bit operands against the fp64 dot product of
     the SAME rounded operands."""
     import ctypes as C
     torch.manual_seed(5)

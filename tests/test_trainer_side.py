@@ -83,7 +83,7 @@ def test_oracle_losses_equal_reference(losses, golden_dir):
 
 @pytest.mark.gpu
 def test_gpu_forward_loss(losses, golden_dir):
-    """ance_b200 forward(): the reference's formula on the sm_100a embeddings (tight), and the reference's value
+    """ance_b200 forward(): the reference's formula on the sm_90a embeddings (tight), and the reference's value
     (loose: a logit is a 768-term dot product of LayerNorm-ed vectors, |q||x| = 768, so the bf16 activation noise of
     tests/test_gpu_encoder.py -- cosine >= 0.9995 -- moves a logit by up to a few units)."""
     from transformers import RobertaConfig

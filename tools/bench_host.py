@@ -4,7 +4,7 @@
   row 2  token-cache reading: ance_b200.data.StridedBatchReader (bulk memmap gather) vs the reference-style
          StreamingDataset(cache, GetProcessingFn) record iterator
   (e)    host k-way merge of per-shard top-k (csrc/merge.cpp)
-Writes one JSON object to stdout (kept in profiles/)."""
+Writes one JSON object to stdout."""
 import argparse
 import json
 import os

@@ -1,4 +1,4 @@
-"""GPU bring-up of the tcgen05 GEMM core: every variant in its own subprocess (a trapped kernel
+"""GPU bring-up of the wgmma GEMM core: every variant in its own subprocess (a trapped kernel
 poisons the CUDA context), results appended to gpurun_out/bringup_gemm.jsonl."""
 import ctypes as C
 import json

@@ -1,4 +1,4 @@
-"""Summarise `ncu --metrics gpu__time_duration.sum --csv` output into shares per kernel (for profiles/)."""
+"""Summarise `ncu --metrics gpu__time_duration.sum --csv` output into shares per kernel."""
 import csv
 import re
 import sys

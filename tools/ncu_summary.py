@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (read here, without a GPU) into a small text file for profiles/."""
+"""Summarise an .ncu-rep (read here, without a GPU) into a small text file."""
 import csv
 import subprocess
 import sys
