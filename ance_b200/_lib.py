@@ -83,6 +83,8 @@ SIGNATURES = {
                                        C.c_void_p, C.c_void_p]),
     "ance_encoder_forward_varlen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                               C.c_void_p, C.c_void_p]),
+    "ance_encoder_forward_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                              C.c_void_p, C.c_void_p]),
     "ance_encoder_set_param": (C.c_int, [C.c_void_p, C.c_char_p, C.c_double]),
     "ance_encoder_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ance_encoder_debug_hidden": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -90,6 +92,8 @@ SIGNATURES = {
     "ance_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "ance_dbg_pack_varlen": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "ance_dbg_pack_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ance_dbg_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                 C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
 }

@@ -18,6 +18,10 @@
 //   o = o*alpha + O_blk in registers; after the last block ctx = o / l  (16-bit)
 // Sequence lengths: a multiple of 128, or a divisor of 128 (then a tile holds 128/L sequences and
 // cross-sequence scores are excluded).  head_dim is fixed at 64 (BERT/RoBERTa-base).
+// Packed variable-length token matrices (kPacked with a row plan): every row r attends to the keys [row_lo[r], row_hi[r])
+// of its own sequence.  kSingle: no sequence straddles a 128-row tile.  Otherwise an item's keys are the contiguous packed
+// rows [kv0, kv0 + 128 nkv) covering every row's own range (tile_kv); the blocks of it outside a row's range are exact
+// no-ops for that row, and the first block inside it takes the two-pass treatment the dense kernel gives block 0.
 #pragma once
 #include "act16.cuh"
 #include "tc05.cuh"
@@ -42,11 +46,13 @@ struct Params {
   int hidden;          // heads * 64
   const float* kbias;  // [n_tokens] additive key bias * log2(e): 0 or -10000*log2e
   float scale_log2;    // log2(e) / sqrt(64)
-  // Variable-length packing (kPacked kernels only; null = uniform L): token row r of a 128-row tile belongs to a sequence
-  // that occupies the tile-local rows [row_lo[r], row_hi[r]) — whole sequences of ANY length <= 128 share a tile, nothing is
-  // padded inside a sequence (kbias is all zero), rows after the last sequence of a tile attend to themselves only.
-  const uint8_t* row_lo;
-  const uint8_t* row_hi;
+  // Variable-length packing (kPacked kernels only; null = uniform L): token row r belongs to a sequence that occupies the
+  // packed rows [row_lo[r], row_hi[r]) — whole sequences share tiles, nothing is padded inside a sequence (kbias is all
+  // zero), rows that belong to no sequence attend to themselves only.
+  const int32_t* row_lo;
+  const int32_t* row_hi;
+  // kPacked && !kSingle: per 128-row tile, (first key row, number of 128-key blocks) of its work items
+  const int2* tile_kv;
 };
 
 struct Smem {
@@ -75,12 +81,12 @@ constexpr int kThreads = 256;   // warp 0 TMA, 1-3 idle, 4-7 the softmax / MMA w
 // Persistent, one CTA per SM.  The CTA walks its work items w = blockIdx.x + n * gridDim.x; the TMA producer runs
 // up to kStages key/value blocks ahead (the HBM latency of a 48 KB Q/K/V fetch is longer than one item's
 // arithmetic); producer and warpgroup derive the block order from the same loop nest.
-// kPacked: L < 128, a tile holds 128/L sequences.  kSingle: L <= 128, one key block per item.
+// kPacked: L < 128, a tile holds 128/L sequences; or a variable-length row plan (p.row_lo).  kSingle: one key block per
+// item (L <= 128, or a plan whose sequences never straddle a tile).
 // FMT: 16-bit format of Q / K / V, of the probabilities P and of the output (act16.cuh).
 template <bool kPacked, bool kSingle, uint32_t FMT>
 __global__ void __launch_bounds__(kThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
-  static_assert(kSingle || !kPacked, "a packed tile has a single key block");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Smem::kBar);
@@ -92,7 +98,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.n_tokens + kTile - 1) / kTile;
   const int total_work = n_tiles * p.heads;
-  const int nkv = (p.L >= kTile) ? p.L / kTile : 1;
+  const int nkv_dense = (p.L >= kTile) ? p.L / kTile : 1;
+  // keys of the items of a tile: first key row, number of 128-key blocks
+  auto kv_of = [&](int tile, int& kv0, int& nkv) {
+    if constexpr (kPacked && !kSingle) {
+      const int2 t = __ldg(p.tile_kv + tile);
+      kv0 = t.x;
+      nkv = t.y;
+    } else {
+      kv0 = (p.L >= kTile) ? (tile * kTile / p.L) * p.L : tile * kTile;
+      nkv = nkv_dense;
+    }
+  };
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmQKV);
@@ -115,7 +132,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
       for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
         const int tile = w / p.heads, h = w - tile * p.heads;
         const int tok0 = tile * kTile;
-        const int kv_tok0 = (p.L >= kTile) ? (tok0 / p.L) * p.L : tok0;
+        int kv_tok0, nkv;
+        kv_of(tile, kv_tok0, nkv);
         for (int j = 0; j < nkv; ++j) {
           if (j == 0) {
             mbar_wait(q_empty, (qc & 1) ^ 1, 10);
@@ -150,8 +168,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
     // additive key bias of block (w2, j2) for key `row` of that block (fetched one block ahead of its use)
     auto load_bias = [&](int w2, int j2) -> float {
       if (w2 >= total_work) return 0.f;
-      const int t0 = (w2 / p.heads) * kTile;
-      const int kt = ((p.L >= kTile) ? (t0 / p.L) * p.L : t0) + j2 * kTile + row;
+      int k0, nk;
+      kv_of(w2 / p.heads, k0, nk);
+      const int kt = k0 + j2 * kTile + row;
       return (kt < p.n_tokens) ? __ldg(p.kbias + kt) : -INFINITY;
     };
     // P (and the output tile) rows in shared memory: 128-byte spans, 16-byte chunk index ^= (row & 7)  (SWIZZLE_128B)
@@ -166,13 +185,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
     for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       const int tile = w / p.heads, h = w - tile * p.heads;
       const int tok0 = tile * kTile;
+      int kv0, nkv;
+      kv_of(tile, kv0, nkv);
       const bool varlen = kPacked && p.row_lo != nullptr;
-      int seq_lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;   // keys of this row's own sequence
+      int seq_lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;   // keys of this row's own sequence, relative to kv0
       int seq_hi = (p.L >= kTile) ? kTile : seq_lo + p.L;
       if (varlen) {
-        seq_lo = __ldg(p.row_lo + tok0 + row);
-        seq_hi = __ldg(p.row_hi + tok0 + row);
+        seq_lo = __ldg(p.row_lo + tok0 + row) - kv0;
+        seq_hi = __ldg(p.row_hi + tok0 + row) - kv0;
       }
+      // end of the whole 32-key chunks of the own sequence (counted from its first key): the keys the dense kernel,
+      // with the sequence at key 0, handles in unmasked chunks
+      const int seq_full = seq_lo + ((seq_hi - seq_lo) & ~31);
       float m_run = -INFINITY, l_run = 0.f;
       float o[kDh];
       if constexpr (!kSingle) {
@@ -194,14 +218,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
         // masked while the row has an unmasked key somewhere: exp2(-10000 log2e + s - m) flushes to zero, as
         // exp(-10000 + s - m) does in the reference's fp32 softmax),  1 = no key masked (no bias term),  2 = general.
         const unsigned mk[4] = {smask[0], smask[1], smask[2], smask[3]};
-        // (variable-length tiles: a row whose sequence fills the whole tile takes the same arithmetic as a full-length
-        // sequence of the dense L = 128 kernel, so that the two paths agree bit for bit)
-        const bool plain = kPacked ? (varlen && seq_lo == 0 && seq_hi == kTile) : ((mk[0] | mk[1] | mk[2] | mk[3]) == 0u);
+        // (variable-length tiles: a row whose sequence covers the whole block takes the same arithmetic as a full-length
+        // sequence of the dense kernel, so that the two paths agree bit for bit)
+        const int bl = seq_lo - j * kTile, bh = seq_hi - j * kTile;   // own keys, relative to this block
+        const int bf = seq_full - j * kTile;
+        const bool plain = kPacked ? (varlen && bl <= 0 && bh >= kTile) : ((mk[0] | mk[1] | mk[2] | mk[3]) == 0u);
         int st[4];
         if (varlen) {   // per row: chunk outside / inside / straddling the boundary of the row's own sequence
+          // (several key blocks: "inside" also needs the chunk's keys to lie in whole 32-key chunks of the sequence, as
+          // the unmasked chunks of the dense kernel do; the others take the dense kernel's partial-chunk arithmetic)
 #pragma unroll
           for (int c = 0; c < 4; ++c)
-            st[c] = (seq_hi <= c * 32 || seq_lo >= c * 32 + 32) ? 0 : (seq_lo <= c * 32 && seq_hi >= c * 32 + 32) ? 1 : 2;
+            st[c] = (bh <= c * 32 || bl >= c * 32 + 32) ? 0 : (bl <= c * 32 && (kSingle ? bh : bf) >= c * 32 + 32) ? 1 : 2;
         } else {
           bool own[4], any_unmasked = false;
 #pragma unroll
@@ -267,7 +295,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
 #pragma unroll
                 for (int i = c; i < c + 32; ++i) {
                   float t = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[i]);
-                  if (kPacked && (i < seq_lo || i >= seq_hi)) t = -INFINITY;
+                  if (kPacked && (i < bl || i >= bh)) t = -INFINITY;
                   v[i] = __float_as_uint(t);
                   mx[i & 3] = fmaxf(mx[i & 3], t);
                 }
@@ -327,8 +355,13 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
                 } else {
 #pragma unroll
                   for (int i = 0; i < 32; i += 2) {
-                    const float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]) + nm;
-                    const float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, sbias[c + i + 1]) + nm;
+                    float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]) + nm;
+                    float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, sbias[c + i + 1]) + nm;
+                    if constexpr (kPacked) {   // other sequences' keys: nothing; keys of whole chunks: unmasked arithmetic
+                      const int k0 = c + i, k1 = c + i + 1;
+                      u0 = (k0 < bl || k0 >= bh) ? -INFINITY : (k0 < bf) ? fmaf(__uint_as_float(v[i]), p.scale_log2, nm) : u0;
+                      u1 = (k1 < bl || k1 >= bh) ? -INFINITY : (k1 < bf) ? fmaf(__uint_as_float(v[i + 1]), p.scale_log2, nm) : u1;
+                    }
                     mu = fmaxf(mu, fmaxf(u0, u1));
                     const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
                     rs_ += p0 + p1;
@@ -346,20 +379,23 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
           // (log2 units) — then, and only then, the warp redoes the block relative to the true maximum.  The softmax is
           // the same function either way (numerator and denominator carry the same factor 2^(m_true - m_ref)).
           const bool optimistic = __all_sync(0xffffffffu, j > 0 && m_run > kRealMax);
+          // (packed tiles: all_skip may differ between the rows of a warp, so the vote is taken by every lane; a skipped
+          // row has over = -inf, and a redo leaves it as it was: m_new = m_run, alpha = 1, P = 0)
           if (optimistic) {
             m_new = m_run;
             alpha = 1.f;
             rsum = 0.f;
+            float over = -INFINITY;
             if (!all_skip) {
-              const float over = exp_pass(m_run, rsum);
-              if (__any_sync(0xffffffffu, over > 8.0f)) {
-                m_new = fmaxf(m_run, m_run + over);
-                alpha = exp2f(m_run - m_new);
-                exp_pass(m_new, rsum);
-              }
+              over = exp_pass(m_run, rsum);
             } else {
               float dummy;
               exp_pass(m_run, dummy);   // (writes the zero P tile; no score reads: every chunk state is 0)
+            }
+            if (__any_sync(0xffffffffu, over > 8.0f)) {
+              m_new = fmaxf(m_run, m_run + over);
+              alpha = exp2f(m_run - m_new);
+              exp_pass(m_new, rsum);
             }
           } else {
             // first block of an item (or no real key seen yet): pass 1 = row max (of the raw scores when `plain`:
@@ -380,7 +416,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
                   for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]) * p.scale_log2);
                 } else {
 #pragma unroll
-                  for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]));
+                  for (int i = 0; i < 32; ++i) {
+                    float t = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]);
+                    if (kPacked && (c + i < bl || c + i >= bh)) t = -INFINITY;
+                    m_blk = fmaxf(m_blk, t);
+                  }
                 }
               }
             }

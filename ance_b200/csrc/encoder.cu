@@ -49,6 +49,8 @@ struct EmbedParams {
   int* err_flag;
   const int32_t* seq_row0;  // variable-length packing: first packed row of sequence b (null: row b*L); only the
                             // len[b] real tokens are written, kbias is left alone (all zero)
+  int long_pad;             // packing: a sequence longer than 128 also writes its padding tokens up to a multiple of
+                            // this many rows (0: none), see pack_chunk
 };
 
 template <int NV, uint32_t FMT>  // H = NV * 256
@@ -78,7 +80,7 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const EmbedParams p) {
   const int len = p.lens ? p.lens[b] : 0;
   const bool varlen = p.seq_row0 != nullptr;
   const size_t row0 = varlen ? static_cast<size_t>(p.seq_row0[b]) : static_cast<size_t>(b) * p.L;
-  const int t_end = varlen ? min(len, p.L) : p.L;
+  const int t_end = !varlen ? p.L : (p.long_pad && len > 128) ? min((len + p.long_pad - 1) / p.long_pad * p.long_pad, p.L) : min(len, p.L);
   for (int t = warp; t < t_end; t += 8) {
     const size_t tok = row0 + t;
     int id = ids[t];
@@ -424,13 +426,14 @@ struct ance_encoder {
   float* kbias = nullptr;
   uint16_t *cls_ctx = nullptr, *cls_x = nullptr;   // [max_seqs, H]: CLS rows gathered for the pruned last layer (varlen)
   int32_t* seq_row0 = nullptr;                     // [max_seqs] varlen plan: first packed row of each sequence
-  uint8_t *row_lo = nullptr, *row_hi = nullptr;    // [max_tokens] varlen plan: own-sequence key range of each packed row
+  int32_t *row_lo = nullptr, *row_hi = nullptr;    // [max_tokens] varlen plan: own-sequence key range of each packed row
+  int2* tile_kv = nullptr;                         // [max_tokens / 128] varlen plan: key blocks of each tile
   float* head_tmp = nullptr;  // [max_seqs, H] fp32
   int* err_flag = nullptr;
   uint16_t* dbg = nullptr;       // [(n_layer+1), max_tokens, H] when debugging
   int dbg_tokens = 0;
   int prune_last_layer = 1;  // last layer: only the CLS rows go through out-proj / FFN (identical result)
-  int varlen_align = 1;      // ance_encoder_forward_varlen: slot alignment inside a tile (1 | 16), see pack_chunk
+  int varlen_align = 1;      // ance_encoder_forward_varlen / _packed: 1 = densest, 16 = exact packing, see pack_chunk
   std::vector<void*> allocs;
 };
 
@@ -540,16 +543,18 @@ int set_attention_attrs() {
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<false, false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<false, true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<true, true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<true, false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   return ANCE_OK;
 }
 
-// n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi) is already on the device, the token
-// matrix has n_tiles * 128 rows and the CLS rows are gathered by index.
+// n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
+// token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
 template <uint32_t FMT>
 int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev, int B, int L,
                  float* out_dev, cudaStream_t st, int n_tiles = 0) {
   const ance_encoder_config& c = e->cfg;
   const bool varlen = n_tiles > 0;
+  const bool varlen_long = varlen && L > attn::kTile;   // sequences may span several tiles: multi-block attention items
   const int M = varlen ? n_tiles * attn::kTile : B * L, H = c.hidden, F = c.ffn;
   int rc;
   if (varlen) {   // rows behind the last sequence of a tile: zeros (finite through every layer), no key bias anywhere
@@ -566,6 +571,7 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   ep.gamma = e->eg; ep.beta = e->eb; ep.eps = c.ln_eps;
   ep.X = e->X; ep.kbias = e->kbias; ep.err_flag = e->err_flag;
   ep.seq_row0 = varlen ? e->seq_row0 : nullptr;
+  ep.long_pad = (varlen_long && e->varlen_align == 16) ? 32 : 0;
   ance::prof_begin(ance::kClsNorm, st);
   switch (H / 256) {
     case 1: embed_ln_kernel<1, FMT><<<B, 256, 0, st>>>(ep); break;
@@ -589,18 +595,20 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
     return ANCE_ERR_CUDA;
   }
   attn::Params ap;
-  ap.n_tokens = M; ap.L = varlen ? 64 : L; ap.heads = c.heads; ap.hidden = H;   // varlen: any L < 128 selects the packed kernel
+  ap.n_tokens = M; ap.L = (varlen && !varlen_long) ? 64 : L; ap.heads = c.heads; ap.hidden = H;   // varlen: any L < 128 selects the packed kernel
   ap.kbias = e->kbias;
   ap.scale_log2 = kLog2e / 8.0f;
   ap.row_lo = varlen ? e->row_lo : nullptr;
   ap.row_hi = varlen ? e->row_hi : nullptr;
+  ap.tile_kv = varlen ? e->tile_kv : nullptr;
   const int attn_work = ((M + 127) / 128) * c.heads;
   const int attn_grid = std::min(attn_work, gemm::sm_count());
   for (int l = 0; l < c.n_layer; ++l) {
     const LayerDev& d = e->layers[l];
     if ((rc = linear<FMT>(e->X, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, e->QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
     ance::prof_begin(ance::kClsAttn, st);
-    if (varlen || L < attn::kTile) attn::attention_kernel<true, true, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
+    if (varlen_long) attn::attention_kernel<true, false, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
+    else if (varlen || L < attn::kTile) attn::attention_kernel<true, true, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
     else if (L == attn::kTile) attn::attention_kernel<false, true, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
     else attn::attention_kernel<false, false, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
     ance::prof_end(ance::kClsAttn, st);
@@ -727,8 +735,9 @@ extern "C" int ance_encoder_create(const ance_encoder_config* cfg, const ance_en
   chk(e->cls_ctx = dev_alloc<uint16_t>(e, T / 16 * H));
   chk(e->cls_x = dev_alloc<uint16_t>(e, T / 16 * H));
   chk(e->seq_row0 = dev_alloc<int32_t>(e, T / 16));
-  chk(e->row_lo = dev_alloc<uint8_t>(e, T));
-  chk(e->row_hi = dev_alloc<uint8_t>(e, T));
+  chk(e->row_lo = dev_alloc<int32_t>(e, T));
+  chk(e->row_hi = dev_alloc<int32_t>(e, T));
+  chk(e->tile_kv = dev_alloc<int2>(e, T / attn::kTile));
   chk(e->head_tmp = dev_alloc<float>(e, T / 16 * H));
   chk(e->err_flag = dev_alloc<int>(e, 1));
   if (!ok || cudaGetLastError() != cudaSuccess) {
@@ -774,30 +783,73 @@ extern "C" int ance_encoder_forward(ance_encoder_t e, const int32_t* ids_dev, co
 }
 
 // ------------------------------------------------------------------------------------------------
-// variable-length forward: whole sequences of any length <= 128 packed into 128-row attention tiles
+// variable-length forward: whole sequences packed into 128-row attention tiles
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// Online best-fit of sequences first .. (in order) into at most cap_tiles tiles of 128 rows: every sequence goes to the
-// fullest tile that still has room for it (all tiles of the chunk stay open, so this packs almost as well as an offline
-// pass).  Stops at the first sequence that fits nowhere, or at max_seqs.  Returns the number of sequences placed.
-// align: every sequence starts at a multiple of `align` rows of its tile (its slot is padded up to a multiple).  With
+struct PackPlan {
+  std::vector<int32_t> row0;     // [placed] first packed row of each sequence
+  std::vector<int32_t> lo, hi;   // [n_tiles * 128] own-sequence key range of every packed row (absolute rows)
+  std::vector<int2> tile_kv;     // [n_tiles] (first key row, number of 128-key blocks) of the tile's attention items
+  int n_tiles = 0;
+};
+
+// Plans sequences first .. (in order) into at most cap_tiles tiles of 128 rows; stops at the first sequence that fits
+// nowhere, or at max_seqs.  Returns the number of sequences placed (a sequence never crosses a chunk of work).
+//
+// Sequences of <= 128 tokens: online best-fit — every sequence goes to the fullest tile that still has room for it (all
+// tiles of the chunk stay open, so this packs almost as well as an offline pass); no sequence straddles a tile.
+// align: every such sequence starts at a multiple of `align` rows of its tile (its slot is padded up to a multiple).  With
 // align = 16 — the K step of a 16-bit wgmma — the P*V accumulation and the softmax row sum of a sequence group their
 // terms exactly as they do at offset 0, so its embedding does not depend on what else is in the tile and equals the dense
 // forward's bit for bit; align = 1 packs ~12 % more real tokens per tile.
-int pack_chunk(const int32_t* lens, int first, int B, int cap_tiles, int max_seqs, int align, std::vector<int32_t>& row0,
-               std::vector<uint8_t>& lo, std::vector<uint8_t>& hi, int* n_tiles_out) {
+//
+// L > 128 (long = more than 128 tokens):
+//   align = 16 (exact): a long sequence starts on a tile boundary and fills ceil(len / 128) consecutive tiles, so its key
+//     blocks are the dense kernel's.  Its rows are padded up to a multiple of 32 with its own padding tokens: the softmax
+//     warp that holds its last rows then holds the same 32 query rows as in the dense forward (the warp votes on a
+//     re-scaling pass together).  Shorter sequences take the best-fit rule above, also in the free rows of a long
+//     sequence's last tile.  Every embedding is bit-identical to the dense forward at the same L.
+//   align = 1 (densest): every sequence starts where the previous one ends; an attention item then reads the keys of every
+//     sequence its tile touches, possibly more than 4 blocks.
+int pack_chunk(const int32_t* lens, int first, int B, int L, int cap_tiles, int max_seqs, int align, PackPlan& plan) {
   constexpr int T = attn::kTile;
+  const bool long_rules = L > T;
   std::vector<int> used;            // rows used per tile
   std::vector<int> head(T + 1, -1); // head[f] = a tile with exactly f free rows (intrusive lists through next[])
   std::vector<int> next;
-  row0.clear();
+  std::vector<int> rows;            // rows computed per placed sequence
+  plan.row0.clear();
   auto push = [&](int tile) { const int f = T - used[tile]; next[tile] = head[f]; head[f] = tile; };
-  int placed = 0;
+  int placed = 0, cursor = 0;
   for (int b = first; b < B && placed < max_seqs; ++b) {
-    const int len = (lens[b] + align - 1) / align * align;   // rows of the slot
+    const int len = lens[b];
+    if (long_rules && align == 1) {   // densest: contiguous
+      if (cursor + len > cap_tiles * T) break;
+      plan.row0.push_back(cursor);
+      rows.push_back(len);
+      cursor += len;
+      ++placed;
+      continue;
+    }
+    if (long_rules && len > T) {      // exact, long: fresh tiles
+      const int n = (len + T - 1) / T;
+      if (static_cast<int>(used.size()) + n > cap_tiles) break;
+      const int r = std::min((len + 31) / 32 * 32, L);
+      const int t0 = static_cast<int>(used.size());
+      for (int k = 0; k < n; ++k) {
+        used.push_back(std::min(T, r - k * T));
+        next.push_back(-1);
+      }
+      if (used.back() < T) push(t0 + n - 1);
+      plan.row0.push_back(t0 * T);
+      rows.push_back(r);
+      ++placed;
+      continue;
+    }
+    const int slot = (len + align - 1) / align * align;   // rows of the slot
     int tile = -1;
-    for (int f = len; f <= T; ++f)   // smallest free space that fits = fullest tile
+    for (int f = slot; f <= T; ++f)   // smallest free space that fits = fullest tile
       if (head[f] >= 0) { tile = head[f]; head[f] = next[tile]; break; }
     if (tile < 0) {
       if (static_cast<int>(used.size()) >= cap_tiles) break;
@@ -805,27 +857,66 @@ int pack_chunk(const int32_t* lens, int first, int B, int cap_tiles, int max_seq
       used.push_back(0);
       next.push_back(-1);
     }
-    row0.push_back(tile * T + used[tile]);
-    used[tile] += len;
+    plan.row0.push_back(tile * T + used[tile]);
+    rows.push_back(len);
+    used[tile] += slot;
     if (used[tile] < T) push(tile);
     ++placed;
   }
-  const int n_tiles = static_cast<int>(used.size());
-  lo.assign(static_cast<size_t>(n_tiles) * T, 0);
-  hi.assign(static_cast<size_t>(n_tiles) * T, 0);
-  for (int r = 0; r < n_tiles * T; ++r) {   // default: a row behind the last sequence of its tile attends to itself
-    lo[r] = static_cast<uint8_t>(r % T);
-    hi[r] = static_cast<uint8_t>(r % T + 1);
+  const int n_tiles = (long_rules && align == 1) ? (cursor + T - 1) / T : static_cast<int>(used.size());
+  plan.lo.resize(static_cast<size_t>(n_tiles) * T);
+  plan.hi.resize(static_cast<size_t>(n_tiles) * T);
+  for (int r = 0; r < n_tiles * T; ++r) {   // default: a row that belongs to no sequence attends to itself
+    plan.lo[r] = r;
+    plan.hi[r] = r + 1;
   }
   for (int i = 0; i < placed; ++i) {
-    const int r0 = row0[i], len = lens[first + i];
-    for (int t = 0; t < len; ++t) {
-      lo[r0 + t] = static_cast<uint8_t>(r0 % T);
-      hi[r0 + t] = static_cast<uint8_t>(r0 % T + len);
+    const int r0 = plan.row0[i], len = lens[first + i];
+    for (int t = 0; t < rows[i]; ++t) {
+      plan.lo[r0 + t] = r0;
+      plan.hi[r0 + t] = r0 + len;
     }
   }
-  *n_tiles_out = n_tiles;
+  plan.tile_kv.resize(n_tiles);
+  for (int t = 0; t < n_tiles; ++t) {   // keys of a tile: from the smallest own-sequence start to the largest end
+    int kv0 = plan.lo[t * T], kv1 = plan.hi[t * T];
+    for (int r = t * T; r < (t + 1) * T; ++r) {
+      kv0 = std::min(kv0, plan.lo[r]);
+      kv1 = std::max(kv1, plan.hi[r]);
+    }
+    plan.tile_kv[t] = make_int2(kv0, (kv1 - kv0 + T - 1) / T);
+  }
+  plan.n_tiles = n_tiles;
   return placed;
+}
+
+int forward_packed_impl(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev, const int32_t* lens_host, int B,
+                        int L, float* out_dev, void* stream) {
+  const ance_encoder_config& c = e->cfg;
+  int dev = -1;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  ANCE_REQUIRE(dev == e->device, "the encoder handle belongs to device %d but device %d is current", e->device, dev);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int cap_tiles = e->max_tokens / attn::kTile, max_seqs = e->max_tokens / 16;
+  PackPlan plan;
+  for (int first = 0; first < B;) {
+    const int n = pack_chunk(lens_host, first, B, L, cap_tiles, max_seqs, e->varlen_align, plan);
+    ANCE_REQUIRE(n > 0, "packed forward: sequence %d (%d tokens) does not fit a handle of max_tokens %d", first,
+                 lens_host[first], e->max_tokens);
+    // the plan arrays are read by the kernels of this chunk only; pageable cudaMemcpyAsync stages them before returning
+    ANCE_CUDA(cudaMemcpyAsync(e->seq_row0, plan.row0.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
+    ANCE_CUDA(cudaMemcpyAsync(e->row_lo, plan.lo.data(), plan.lo.size() * 4, cudaMemcpyHostToDevice, st));
+    ANCE_CUDA(cudaMemcpyAsync(e->row_hi, plan.hi.data(), plan.hi.size() * 4, cudaMemcpyHostToDevice, st));
+    ANCE_CUDA(cudaMemcpyAsync(e->tile_kv, plan.tile_kv.data(), plan.tile_kv.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+    const int32_t* ids = ids_dev + static_cast<size_t>(first) * L;
+    float* out = out_dev + static_cast<size_t>(first) * c.hidden;
+    const int rc = (e->fmt == tc05::kFmtBF16)
+                       ? forward_impl<tc05::kFmtBF16>(e, ids, lens_dev + first, nullptr, n, L, out, st, plan.n_tiles)
+                       : forward_impl<tc05::kFmtF16>(e, ids, lens_dev + first, nullptr, n, L, out, st, plan.n_tiles);
+    if (rc) return rc;
+    first += n;
+  }
+  return ANCE_OK;
 }
 
 }  // namespace
@@ -836,12 +927,33 @@ extern "C" int ance_dbg_pack_varlen(const int32_t* lens_host, int B, int max_tok
   ANCE_REQUIRE(lens_host && row0_out && n_placed && n_tiles && B > 0 && max_tokens >= attn::kTile, "ance_dbg_pack_varlen: bad arguments");
   ANCE_REQUIRE(align == 1 || align == 16, "ance_dbg_pack_varlen: align must be 1 or 16");
   for (int b = 0; b < B; ++b) ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= attn::kTile, "ance_dbg_pack_varlen: length %d out of range", lens_host[b]);
-  std::vector<int32_t> row0;
-  std::vector<uint8_t> lo, hi;
-  *n_placed = pack_chunk(lens_host, 0, B, max_tokens / attn::kTile, max_tokens / 16, align, row0, lo, hi, n_tiles);
-  memcpy(row0_out, row0.data(), row0.size() * 4);
-  if (lo_out) memcpy(lo_out, lo.data(), lo.size());
-  if (hi_out) memcpy(hi_out, hi.data(), hi.size());
+  PackPlan plan;
+  *n_placed = pack_chunk(lens_host, 0, B, attn::kTile, max_tokens / attn::kTile, max_tokens / 16, align, plan);
+  *n_tiles = plan.n_tiles;
+  memcpy(row0_out, plan.row0.data(), plan.row0.size() * 4);
+  for (size_t r = 0; r < plan.lo.size(); ++r) {   // tile-local
+    const int t0 = static_cast<int>(r / attn::kTile) * attn::kTile;
+    if (lo_out) lo_out[r] = static_cast<uint8_t>(plan.lo[r] - t0);
+    if (hi_out) hi_out[r] = static_cast<uint8_t>(plan.hi[r] - t0);
+  }
+  return ANCE_OK;
+}
+
+extern "C" int ance_dbg_pack_packed(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
+                                    int32_t* lo_out, int32_t* hi_out, int32_t* tile_kv_out, int* n_placed, int* n_tiles) {
+  ANCE_REQUIRE(lens_host && row0_out && n_placed && n_tiles && B > 0, "ance_dbg_pack_packed: bad arguments");
+  ANCE_REQUIRE(L > 0 && L <= 512 && max_tokens >= (L + attn::kTile - 1) / attn::kTile * attn::kTile,
+               "ance_dbg_pack_packed: need 0 < L <= 512 and max_tokens >= L rounded up to 128 (L = %d, max_tokens = %d)", L, max_tokens);
+  ANCE_REQUIRE(align == 1 || align == 16, "ance_dbg_pack_packed: align must be 1 or 16");
+  for (int b = 0; b < B; ++b) ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= L, "ance_dbg_pack_packed: length %d outside [1, %d]", lens_host[b], L);
+  PackPlan plan;
+  const int mt = max_tokens / attn::kTile * attn::kTile;
+  *n_placed = pack_chunk(lens_host, 0, B, L, mt / attn::kTile, mt / 16, align, plan);
+  *n_tiles = plan.n_tiles;
+  memcpy(row0_out, plan.row0.data(), plan.row0.size() * 4);
+  if (lo_out) memcpy(lo_out, plan.lo.data(), plan.lo.size() * 4);
+  if (hi_out) memcpy(hi_out, plan.hi.data(), plan.hi.size() * 4);
+  if (tile_kv_out) memcpy(tile_kv_out, plan.tile_kv.data(), plan.tile_kv.size() * sizeof(int2));
   return ANCE_OK;
 }
 
@@ -855,29 +967,22 @@ extern "C" int ance_encoder_forward_varlen(ance_encoder_t e, const int32_t* ids_
   ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "ance_encoder_forward_varlen: L = %d exceeds max_position_embeddings %d", L, c.max_pos);
   for (int b = 0; b < B; ++b)
     ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= L, "ance_encoder_forward_varlen: length %d of sequence %d outside [1, %d]", lens_host[b], b, L);
-  int dev = -1;
-  ANCE_CUDA(cudaGetDevice(&dev));
-  ANCE_REQUIRE(dev == e->device, "ance_encoder_forward_varlen: the handle belongs to device %d but device %d is current", e->device, dev);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int cap_tiles = e->max_tokens / attn::kTile, max_seqs = e->max_tokens / 16;
-  std::vector<int32_t> row0;
-  std::vector<uint8_t> lo, hi;
-  for (int first = 0; first < B;) {
-    int n_tiles = 0;
-    const int n = pack_chunk(lens_host, first, B, cap_tiles, max_seqs, e->varlen_align, row0, lo, hi, &n_tiles);
-    // the plan arrays are read by the kernels of this chunk only; pageable cudaMemcpyAsync stages them before returning
-    ANCE_CUDA(cudaMemcpyAsync(e->seq_row0, row0.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
-    ANCE_CUDA(cudaMemcpyAsync(e->row_lo, lo.data(), lo.size(), cudaMemcpyHostToDevice, st));
-    ANCE_CUDA(cudaMemcpyAsync(e->row_hi, hi.data(), hi.size(), cudaMemcpyHostToDevice, st));
-    const int32_t* ids = ids_dev + static_cast<size_t>(first) * L;
-    float* out = out_dev + static_cast<size_t>(first) * c.hidden;
-    const int rc = (e->fmt == tc05::kFmtBF16)
-                       ? forward_impl<tc05::kFmtBF16>(e, ids, lens_dev + first, nullptr, n, L, out, st, n_tiles)
-                       : forward_impl<tc05::kFmtF16>(e, ids, lens_dev + first, nullptr, n, L, out, st, n_tiles);
-    if (rc) return rc;
-    first += n;
-  }
-  return ANCE_OK;
+  return forward_packed_impl(e, ids_dev, lens_dev, lens_host, B, L, out_dev, stream);
+}
+
+extern "C" int ance_encoder_forward_packed(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
+                                           const int32_t* lens_host, int B, int L, float* out_dev, void* stream) {
+  ANCE_REQUIRE(e != nullptr, "ance_encoder_forward_packed: null handle");
+  ANCE_REQUIRE(ids_dev && lens_dev && lens_host && out_dev, "ance_encoder_forward_packed: null buffer");
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= 512, "ance_encoder_forward_packed: need B > 0 and 0 < L <= 512 (got B = %d, L = %d)", B, L);
+  const ance_encoder_config& c = e->cfg;
+  ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "ance_encoder_forward_packed: L = %d exceeds max_position_embeddings %d", L, c.max_pos);
+  ANCE_REQUIRE(e->max_tokens >= (L + attn::kTile - 1) / attn::kTile * attn::kTile,
+               "ance_encoder_forward_packed: L = %d needs a handle of max_tokens >= %d (got %d)", L,
+               (L + attn::kTile - 1) / attn::kTile * attn::kTile, e->max_tokens);
+  for (int b = 0; b < B; ++b)
+    ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= L, "ance_encoder_forward_packed: length %d of sequence %d outside [1, %d]", lens_host[b], b, L);
+  return forward_packed_impl(e, ids_dev, lens_dev, lens_host, B, L, out_dev, stream);
 }
 
 extern "C" int ance_encoder_set_param(ance_encoder_t e, const char* name, double value) {

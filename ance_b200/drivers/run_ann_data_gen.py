@@ -171,6 +171,10 @@ class B200Backend:
         per = max(B, (args.encode_batch_tokens // L) // B * B) if multi else max(1, args.encode_batch_tokens // L)
         bucketed = self.mask_mode != "nonzero" and not multi and getattr(args, "length_buckets", True)
         varlen = bucketed and L <= 128 and getattr(args, "varlen", True) and hasattr(self.model, "encode_lens_varlen")
+        # MaxP documents and DPR passages / questions: the packed forward in exact mode (align 16), whose embeddings are
+        # bit-identical to the padded forward's
+        packed = getattr(args, "varlen", True) and hasattr(
+            self.model, "query_emb_packed" if self.mask_mode == "nonzero" else "encode_lens_multi_chunk_packed")
         if bucketed:
             per *= 8   # every length bucket of a super-batch should still fill the GPU (the encoder re-splits by tokens)
         reader = StridedBatchReader(cache, per, rank=rank, world_size=W)
@@ -189,12 +193,19 @@ class B200Backend:
                 ids_d = ids.to(self.device, non_blocking=True)
                 lens_d = lens.to(self.device, non_blocking=True)
                 out = rows[pos:pos + ids.shape[0] * C]
-                if self.mask_mode == "nonzero":
+                if self.mask_mode == "nonzero" and packed:
+                    fn = self.model.query_emb_packed if is_query else self.model.body_emb_packed
+                    out.copy_(fn(ids_d, align=16, ids_host=ids))
+                    i = idx.numpy()
+                elif self.mask_mode == "nonzero":
                     fn = self.model.query_emb if is_query else self.model.body_emb
                     out.copy_(fn(ids_d, ids_d != 0))
                     i = idx.numpy()
                 elif multi:
-                    e = self.model.encode_lens_multi_chunk(ids_d, lens_d)
+                    if packed:
+                        e = self.model.encode_lens_multi_chunk_packed(ids_d, lens_d, lens_host=lens, align=16)
+                    else:
+                        e = self.model.encode_lens_multi_chunk(ids_d, lens_d)
                     e, i = rows_from_batches(e, idx.numpy(), B)
                     out.copy_(e)
                 elif varlen:
@@ -591,7 +602,9 @@ def get_arguments(argv=None):
                         "packs ~12 %% more real tokens per tile, embeddings agree to fp32 summation order")
     p.add_argument("--no_varlen", dest="varlen", action="store_false",
                    help="L <= 128 caches: group sequences into padded length buckets instead of packing whole sequences of any "
-                        "length into 128-token attention tiles (same embeddings up to fp32 summation order)")
+                        "length into 128-token attention tiles (same embeddings up to fp32 summation order); MaxP documents "
+                        "and DPR passages / questions: encode every sequence at the cache's padded length instead of packing "
+                        "the real tokens (bit-identical embeddings either way)")
     p.add_argument("--no_length_buckets", dest="length_buckets", action="store_false",
                    help="encode every sequence at the cache's full padded length (the reference's behaviour); by default "
                         "sequences are grouped by the smallest supported padded length, which yields the same embeddings")

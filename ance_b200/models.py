@@ -186,6 +186,18 @@ def _forward_varlen(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Opti
                     out: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
     """ids int32 [B, L <= 128] CUDA, lens int32 [B] CUDA (+ the same lengths on the host, else they are copied back):
     only the real tokens are computed (ance_encoder_forward_varlen).  -> fp32 [B, H]."""
+    return _forward_plan(self, self.lib.ance_encoder_forward_varlen, ids, lens, lens_host, out, align)
+
+
+def _forward_packed(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
+                    out: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
+    """ids int32 [B, L <= 512] CUDA, lens int32 [B] CUDA, each in [1, L] (+ the same lengths on the host, else they are
+    copied back): only the real tokens are computed, sequences of up to 512 tokens (ance_encoder_forward_packed).
+    align = 16: bit-identical to forward() at the same L; align = 1: densest packing.  -> fp32 [B, H]."""
+    return _forward_plan(self, self.lib.ance_encoder_forward_packed, ids, lens, lens_host, out, align)
+
+
+def _forward_plan(self, entry, ids, lens, lens_host, out, align):
     B, L = ids.shape
     if out is None:
         out = torch.empty((B, self.hidden_size), dtype=torch.float32, device=ids.device)
@@ -198,12 +210,13 @@ def _forward_varlen(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Opti
         raise ValueError("lens_host must be a CPU tensor [B]")
     self.set_param("varlen_align", align)
     with torch.cuda.device(ids.device):
-        _lib.check(self.lib.ance_encoder_forward_varlen(self.h, ids.data_ptr(), lens.data_ptr(), lens_host.data_ptr(), B, L,
-                                                        out.data_ptr(), _lib.current_stream()))
+        _lib.check(entry(self.h, ids.data_ptr(), lens.data_ptr(), lens_host.data_ptr(), B, L, out.data_ptr(),
+                         _lib.current_stream()))
     return out
 
 
 _CudaEncoder.forward_varlen = _forward_varlen
+_CudaEncoder.forward_packed = _forward_packed
 
 
 class _B200Encoder(nn.Module):
@@ -356,6 +369,14 @@ class RobertaDot_NLL_LN(_B200Encoder):
         return self._encoder(ids_i32.device).forward_varlen(ids_i32.contiguous(), lens_i32.contiguous(), lens_host, out=out,
                                                             align=align)
 
+    def encode_lens_packed(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
+                           out: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
+        """encode_lens at the cost of the REAL tokens only, for any L <= 512 (lengths in [1, L]).  align = 16: bit-identical
+        to encode_lens at the same L, whatever else is in the batch; align = 1: densest packing, equal up to fp32
+        summation order.  L <= 128 is encode_lens_varlen."""
+        return self._encoder(ids_i32.device).forward_packed(ids_i32.contiguous(), lens_i32.contiguous(), lens_host, out=out,
+                                                            align=align)
+
     def encode_lens_bucketed(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, min_bucket: int = 16,
                              out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Same result as encode_lens, without the FLOPs of all-padding tails: sequences are grouped by the
@@ -415,6 +436,50 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
         emb = self._encoder(ids_i32.device).forward(ids_i32.reshape(B * cf, seq).contiguous(), clen.contiguous(), None)
         return emb.reshape(B, cf, emb.shape[-1])
 
+    def encode_lens_multi_chunk_packed(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor,
+                                       lens_host: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
+        """encode_lens_multi_chunk (same [B, chunks, 768]) at the cost of the real tokens: the chunks with tokens go through
+        the packed forward (align as in encode_lens_packed; 16 = bit-identical); an all-padding chunk (length 0, every id
+        pad_id, as the token caches store them) gets the one vector such a chunk has, computed once per encoder and
+        weights by the dense forward; any other empty chunk is encoded densely."""
+        B, full = ids_i32.shape
+        cf = full // self.base_len
+        seq = full // cf
+        dev = ids_i32.device
+        if lens_host is None:
+            lens_host = lens_i32.cpu()
+        lh = lens_host.to(torch.int64).reshape(B)
+        clen = (lh[:, None] - torch.arange(cf, dtype=torch.int64)[None, :] * seq).clamp_(0, seq).reshape(-1)
+        ids2 = ids_i32.reshape(B * cf, seq).contiguous()
+        enc = self._encoder(dev)
+        out = torch.empty((B * cf, 768), dtype=torch.float32, device=dev)
+        real = torch.nonzero(clen > 0).flatten()
+        if real.numel() == B * cf:
+            return enc.forward_packed(ids2, clen.to(torch.int32).to(dev), clen.to(torch.int32), out=out,
+                                      align=align).reshape(B, cf, 768)
+        if real.numel():
+            rl = clen[real].to(torch.int32)
+            rd = real.to(dev)
+            out[rd] = enc.forward_packed(ids2[rd].contiguous(), rl.to(dev), rl, align=align)
+        empty = torch.nonzero(clen == 0).flatten().to(dev)
+        allpad = (ids2[empty] == self.config.pad_token_id).all(dim=1).cpu()
+        pad_rows, other = empty[allpad.to(dev)], empty[~allpad.to(dev)]
+        if pad_rows.numel():
+            out[pad_rows] = self._allpad_row(enc, seq)
+        if other.numel():
+            out[other] = enc.forward(ids2[other].contiguous(), torch.zeros(other.numel(), dtype=torch.int32, device=dev),
+                                     None)
+        return out.reshape(B, cf, 768)
+
+    def _allpad_row(self, enc, seq: int) -> torch.Tensor:
+        """The embedding of an all-padding chunk of `seq` tokens (dense forward), cached on the encoder handle, which is
+        rebuilt whenever the weights change."""
+        cache = enc.__dict__.setdefault("_allpad", {})
+        if seq not in cache:
+            ids = torch.full((1, seq), self.config.pad_token_id, dtype=torch.int32, device=enc.device)
+            cache[seq] = enc.forward(ids, torch.zeros(1, dtype=torch.int32, device=enc.device), None)[0]
+        return cache[seq]
+
 
 # ---------------------------------------------------------------------------------------------
 # dpr
@@ -462,6 +527,39 @@ class BiEncoder(_B200Encoder):
 
     def body_emb(self, input_ids, attention_mask):
         return self._emb("ctx", self.ctx_model, input_ids, attention_mask)
+
+    def _emb_packed(self, name, backbone, input_ids, align, ids_host):
+        """Same result as _emb(..., input_ids != 0) (DPR_data.py:283 mask) at the cost of the real tokens: rows whose
+        nonzero ids form a non-empty prefix go through the packed forward, the others through the dense one.  The lengths
+        are read from `ids_host` (the host copy of input_ids; copied back when not given)."""
+        if input_ids.device.type != "cuda":
+            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
+        ids = input_ids.to(torch.int32).contiguous()
+        B, L = ids.shape
+        nz = (ids_host if ids_host is not None else input_ids.cpu()).reshape(B, L) != 0
+        lens = nz.sum(dim=1)
+        ok = (nz == (torch.arange(L)[None, :] < lens[:, None])).all(dim=1) & (lens > 0)
+        enc = self._enc_for(name, backbone, _lib.ANCE_ARCH_BERT, self.dims.num_attention_heads, 0, None, ids.device)
+        lens32 = lens.to(torch.int32)
+        if bool(ok.all()):
+            return enc.forward_packed(ids, lens32.to(ids.device), lens32, align=align)
+        out = torch.empty((B, self.dims.hidden_size), dtype=torch.float32, device=ids.device)
+        sel, rest = torch.nonzero(ok).flatten(), torch.nonzero(~ok).flatten()
+        if sel.numel():
+            sd = sel.to(ids.device)
+            out[sd] = enc.forward_packed(ids[sd].contiguous(), lens32[sel].to(ids.device), lens32[sel].contiguous(),
+                                         align=align)
+        rd = rest.to(ids.device)
+        out[rd] = enc.forward(ids[rd].contiguous(), None, (ids[rd] != 0).to(torch.uint8).contiguous())
+        return out
+
+    def query_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
+        """query_emb(input_ids, input_ids != 0) computing the real tokens only (align: see encode_lens_packed)."""
+        return self._emb_packed("question", self.question_model, input_ids, align, ids_host)
+
+    def body_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
+        """body_emb(input_ids, input_ids != 0) computing the real tokens only (align: see encode_lens_packed)."""
+        return self._emb_packed("ctx", self.ctx_model, input_ids, align, ids_host)
 
     @torch.no_grad()
     def forward(self, query_ids, attention_mask_q, input_ids_a=None, attention_mask_a=None, input_ids_b=None,

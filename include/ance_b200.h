@@ -163,11 +163,21 @@ int ance_encoder_forward(ance_encoder_t enc, const int32_t* ids_dev, const int32
  * is bit-identical to ance_encoder_forward and independent of the batch composition, at ~12 % fewer real tokens per tile. */
 int ance_encoder_forward_varlen(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev,
                                 const int32_t* lens_host, int B, int L, float* out_dev, void* stream);
+/* The same padding-free forward for any 0 < L <= 512 (within max_position_embeddings; the handle needs max_tokens >= L
+ * rounded up to 128).  lens_dev / lens_host as above, each length in [1, L] (else ANCE_ERR_INVALID).  L <= 128 is
+ * ance_encoder_forward_varlen.  For L > 128 sequences may span several tiles; the attention of a tile reads the keys of
+ * every sequence it holds and skips, per row, the blocks outside the row's own sequence.  "varlen_align" = 16 (exact): a
+ * sequence longer than 128 tokens starts on a tile boundary and fills ceil(len / 128) tiles (its rows padded to a multiple
+ * of 32 with its own padding tokens), shorter ones start at a multiple of 16 rows of a tile; every embedding is
+ * bit-identical to ance_encoder_forward at the same L, whatever else is in the batch.  "varlen_align" = 1 (densest): every
+ * sequence starts where the previous one ends; the embeddings equal the dense forward's up to fp32 summation order. */
+int ance_encoder_forward_packed(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev,
+                                const int32_t* lens_host, int B, int L, float* out_dev, void* stream);
 /* Tunables: "prune_last_layer" (default 1): in the last layer only token 0 of every sequence is read
  * downstream, so out-projection / FFN / LayerNorm run on those rows only (result-identical; bench.py reports
  * the executed FLOPs beside the algorithmic ones).  "ln_rows_per_warp" (1, 2, 4, or 3 = two rows held packed; default 2, process-wide): rows a warp
  * of the LayerNorm kernel normalises side by side (bit-identical results; default 2).  "varlen_align" (1 | 16):
- * see ance_encoder_forward_varlen. */
+ * see ance_encoder_forward_varlen and ance_encoder_forward_packed. */
 int ance_encoder_set_param(ance_encoder_t enc, const char* name, double value);
 /* Input / output validation, deferred so that forward stays asynchronous: synchronises `stream` and returns
  * ANCE_ERR_INVALID if any forward since the last check saw a token id outside [0, vocab_size) or a position
@@ -201,6 +211,12 @@ int ance_profile_read(double* ms_by_class, int64_t* launches_by_class, int n, in
  * key range of every packed row (may be null). */
 int ance_dbg_pack_varlen(const int32_t* lens_host, int B, int max_tokens, int align, int32_t* row0_out, uint8_t* lo_out,
                          uint8_t* hi_out, int* n_placed, int* n_tiles);
+/* Host-only: the plan ance_encoder_forward_packed makes for the first chunk of lens_host[0..B) at length L: row0_out[i] as
+ * above, lo/hi_out [*n_tiles * 128] = own-sequence key range of every packed row in absolute packed rows (a row of no
+ * sequence: [r, r + 1)), tile_kv_out [*n_tiles * 2] = (first key row, number of 128-key blocks) of each tile's attention
+ * items.  The three arrays may be null. */
+int ance_dbg_pack_packed(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
+                         int32_t* lo_out, int32_t* hi_out, int32_t* tile_kv_out, int* n_placed, int* n_tiles);
 int ance_dbg_gemm(const void* A_dev, const void* B_dev, int M, int N, int K, int fmt, int variant,
                   const float* bias_dev, const void* residual_bf16_dev, int act, void* C_bf16_dev,
                   float* C_f32_dev, void* stream);
