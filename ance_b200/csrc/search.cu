@@ -160,14 +160,18 @@ __global__ void finalize_mean_kernel(const double* __restrict__ sums, int64_t n,
 // ------------------------------------------------------------------------------------------------
 // 2. coarse pass epilogue: per-query running top-k' over the swept corpus tiles
 // ------------------------------------------------------------------------------------------------
-template <int BN, int CAP>
+// kStream = false: compaction holds the reservoir in registers (CAP / 32 keys and ids per lane; CAP <= 2048).
+// kStream = true (EpTopKWide, reservoirs of 8192 for k > 512): compaction streams over the reservoir in memory with an
+// 8-bit-digit radix select whose histograms live in the epilogue's shared memory (one 256-bin histogram per epilogue
+// warp), so no register array grows with CAP.
+template <int BN, int CAP, bool kStream = false>
 struct EpTopK {
   static constexpr uint64_t kHintA = tc05::kEvictLast;   // query tile: re-read for every corpus tile
   static constexpr uint64_t kHintB = tc05::kEvictNormal;  // corpus rows: every concurrently sweeping CTA pair re-reads
                                                           // the same tile from L2 (EVICT_FIRST would make each pair
                                                           // stream the whole operand from HBM by itself)
-  static constexpr int kSlots = CAP / 32;
-  static constexpr int kSmemBytes = 0;
+  static constexpr int kEpiWarps = 4;   // the coarse pass launches 4 epilogue warps (launch_coarse)
+  static constexpr int kSmemBytes = kStream ? kEpiWarps * 256 * 4 : 0;
   struct Params {
     float* scratch_sc;  // [gridDim.x * 128 * CAP] reservoir scores
     int* scratch_id;    // [gridDim.x * 128 * CAP] reservoir rows
@@ -198,7 +202,13 @@ struct EpTopK {
   // Warp-cooperative exact selection of the best kprime entries of lane `src`'s reservoir
   // (radix select on the order-preserving key, stable compaction: among equal scores the earlier
   // = lower row wins).  Afterwards src.cnt = kprime and src.thr = kprime-th best coarse score.
-  __device__ __forceinline__ void compact(int kprime, int src, int lane) {
+  __device__ __forceinline__ void compact(int kprime, int src, const gemm::EpiCtx& cx) {
+    if constexpr (kStream) compact_stream(kprime, src, cx);
+    else compact_regs(kprime, src, cx.lane);
+  }
+
+  __device__ __forceinline__ void compact_regs(int kprime, int src, int lane) {
+    constexpr int kSlots = CAP / 32;
     const int n = __shfl_sync(0xffffffffu, cnt, src);
     float* s_sc = shfl_ptr(sc, src);
     int* s_id = shfl_ptr(id, src);
@@ -248,6 +258,91 @@ struct EpTopK {
     }
   }
 
+  // Same contract as compact_regs, for reservoirs too large for registers.  Four passes over lane `src`'s reservoir
+  // build 8-bit digit histograms (most significant digit first, only keys that match the digits chosen so far) and pick
+  // the digit that holds the kprime-th best key; a fifth pass compacts in place, stably.  In place is safe: every lane
+  // reads its entry of a 32-entry chunk before any lane writes (the ballots order them), and the write position never
+  // exceeds the read position.
+  __device__ __forceinline__ void compact_stream(int kprime, int src, const gemm::EpiCtx& cx) {
+    const int lane = cx.lane;
+    const int n = __shfl_sync(0xffffffffu, cnt, src);
+    float* s_sc = shfl_ptr(sc, src);
+    int* s_id = shfl_ptr(id, src);
+    uint32_t* hist = reinterpret_cast<uint32_t*>(cx.ep_smem) + cx.epi_warp * 256;
+    uint32_t prefix = 0;
+    int remaining = kprime;   // keys still to select among those that match `prefix`
+#pragma unroll 1
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int b = lane; b < 256; b += 32) hist[b] = 0u;
+      __syncwarp();
+      const uint32_t hmask = (shift == 24) ? 0u : ~((1u << (shift + 8)) - 1u);   // the digits already chosen
+      for (int i = lane; i < n; i += 32) {
+        const uint32_t key = f2ord(s_sc[i]);
+        if ((key & hmask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+      }
+      __syncwarp();
+      // lane l owns digits 255 - 8l down to 248 - 8l: an exclusive scan over lanes counts the keys of larger digits
+      uint32_t c[8];
+      int sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        c[j] = hist[255 - (lane * 8 + j)];
+        sum += static_cast<int>(c[j]);
+      }
+      int incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      const int excl = incl - sum;
+      const unsigned owner = __ballot_sync(0xffffffffu, excl < remaining && remaining <= incl);
+      const int ol = __ffs(owner) - 1;
+      int digit = -1, above = 0, acc = excl;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        if (digit < 0 && acc + static_cast<int>(c[j]) >= remaining) {
+          digit = 255 - (lane * 8 + j);
+          above = acc;
+        }
+        acc += static_cast<int>(c[j]);
+      }
+      digit = __shfl_sync(0xffffffffu, digit, ol);
+      above = __shfl_sync(0xffffffffu, above, ol);
+      prefix |= static_cast<uint32_t>(digit) << shift;
+      remaining -= above;
+      __syncwarp();
+    }
+    const uint32_t T = prefix;   // the kprime-th best key; keep every larger key and the first `remaining` equal ones
+    const unsigned lt = (1u << lane) - 1u;
+    int base = 0, eq_seen = 0;
+#pragma unroll 1
+    for (int i0 = 0; i0 < n; i0 += 32) {
+      const int i = i0 + lane;
+      const bool v = i < n;
+      const float s = v ? s_sc[i] : 0.f;
+      const int r = v ? s_id[i] : 0;
+      const uint32_t key = f2ord(s);
+      const bool gt = v && key > T, eq = v && key == T;
+      const unsigned eqm = __ballot_sync(0xffffffffu, eq);
+      const bool keep = gt || (eq && (eq_seen + __popc(eqm & lt)) < remaining);
+      const unsigned km = __ballot_sync(0xffffffffu, keep);
+      __syncwarp();   // every read of this chunk before any write into it
+      if (keep) {
+        const int pos = base + __popc(km & lt);
+        s_sc[pos] = s;
+        s_id[pos] = r;
+      }
+      base += __popc(km);
+      eq_seen += __popc(eqm);
+    }
+    __syncwarp();
+    if (lane == src) {
+      cnt = kprime;
+      thr = ord2f(T);
+    }
+  }
+
   __device__ __forceinline__ void tile(const Params& p, const gemm::WorkShape&, const gemm::EpiCtx& cx,
                                        uint32_t tacc, int nb) {
 #pragma unroll 1
@@ -274,7 +369,7 @@ struct EpTopK {
       while (need) {
         const int src = __ffs(need) - 1;
         need &= need - 1;
-        compact(p.kprime, src, cx.lane);
+        compact(p.kprime, src, cx);
       }
     }
   }
@@ -287,7 +382,7 @@ struct EpTopK {
     while (need) {
       const int src = __ffs(need) - 1;
       need &= need - 1;
-      compact(p.kprime, src, cx.lane);
+      compact(p.kprime, src, cx);
     }
     for (int l = 0; l < 32; ++l) {
       const int row = cx.row0 + cx.quad * 32 + l;
@@ -528,8 +623,9 @@ __global__ void __launch_bounds__(256) rescore_kernel(const RescoreParams p) {
 // 4. exact brute force (fallback for uncertified queries, and the validation path)
 // ------------------------------------------------------------------------------------------------
 constexpr int kExQB = 4;       // queries per block
-constexpr int kExBuf = 1024;   // reservoir keys per query
 constexpr int kExRound = 16;   // rows per warp between reservoir checks
+// reservoir keys per query: must hold k + nwarps * kExRound (8 warps): 1024 for k <= 512, 4096 for k <= 2048
+constexpr int kExBufSmall = 1024, kExBufLarge = 4096;
 
 struct ExactParams {
   const float* Q;
@@ -540,11 +636,12 @@ struct ExactParams {
   int q_base;
   const int* nq_dev;     // number of queries on the device (null = use nq)
   int nq;
-  int k;                 // <= 512
+  int k;                 // <= 2048
   int n_chunks;
   uint64_t* chunk_keys;  // [nq_cap * n_chunks * k]
 };
 
+template <int kExBuf>
 __global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
   extern __shared__ __align__(16) uint8_t ex_smem[];
   uint64_t* buf = reinterpret_cast<uint64_t*>(ex_smem);              // [kExQB][kExBuf]
@@ -629,7 +726,7 @@ __global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
   }
 }
 
-constexpr int kMergeBuf = 4096;
+constexpr int kMergeBuf = 4096;   // > k: every round merges at least kMergeBuf - k new keys into the best k
 
 __global__ void __launch_bounds__(256) exact_merge_kernel(const ExactParams p, float* D, int64_t* I, int out_k,
                                                           int64_t row_offset) {
@@ -711,6 +808,14 @@ struct ance_index {
 namespace {
 
 constexpr int kMaxPace = 256;
+// k <= 512 keeps reservoirs of 1024 / 2048 (k' <= 992).  512 < k <= kMaxK takes the large-k path: reservoirs of
+// kWideCap, k' in [kWideKPrimeMin, kWideKPrimeMax], at most kWideSortKeys candidates per query (the rescore sorts them in
+// shared memory), queries in blocks of at most kWideQBlock so that the workspace does not grow with nq.
+constexpr int kMaxK = 2048;
+constexpr int kWideCap = 8192;
+constexpr int kWideKPrimeMin = 1024, kWideKPrimeMax = 4096;
+constexpr int kWideSortKeys = 8192;
+constexpr int kWideQBlock = 16384;
 constexpr int kCntQueryErr = 6, kCntRowErr = 7, kNumCounters = 8;
 
 template <class T>
@@ -757,7 +862,7 @@ int check_handle_device(const ance_index* ix, const char* who) {
 template <int BN, int STAGES, int CG, int CAP, uint32_t FMT>
 int launch_coarse(ance_index* ix, const uint16_t* Q16, int64_t nq, int kprime, int out_cap, const float* thr_init,
                   int n_splits_req, int* n_splits_out, cudaStream_t st) {
-  using Ep = EpTopK<BN, CAP>;
+  using Ep = EpTopK<BN, CAP, (CAP > 2048)>;   // CAP > 2048: EpTopKWide (streaming compaction)
   const int N = static_cast<int>(ix->n);
   gemm::WorkShape ws = gemm::make_shape(static_cast<int>(nq), N, ix->dim, BN, CG, n_splits_req);
   *n_splits_out = ws.n_splits;
@@ -772,10 +877,11 @@ int launch_coarse(ance_index* ix, const uint16_t* Q16, int64_t nq, int kprime, i
   }
   const int ctas = (ix->max_ctas > 0 ? ix->max_ctas : gemm::sm_count());
   size_t se = ix->scratch_elems;
-  int rc = ensure(&ix->scratch_sc, &se, static_cast<size_t>(ctas) * gemm::BM * 2048);
+  const size_t res = static_cast<size_t>(ctas) * gemm::BM * std::max(CAP, 2048);
+  int rc = ensure(&ix->scratch_sc, &se, res);
   if (rc) return rc;
   se = ix->scratch_elems;
-  rc = ensure(&ix->scratch_id, &se, static_cast<size_t>(ctas) * gemm::BM * 2048);
+  rc = ensure(&ix->scratch_id, &se, res);
   if (rc) return rc;
   ix->scratch_elems = se;
   const size_t slots = static_cast<size_t>(nq) * ws.n_splits;
@@ -820,6 +926,8 @@ int launch_coarse(ance_index* ix, const uint16_t* Q16, int64_t nq, int kprime, i
 }
 
 constexpr int kExactBatch = 1024;  // queries per brute-force pass (bounds the chunk_keys scratch)
+// k > 512: fewer queries per pass, so that chunk_keys (batch * n_chunks * k * 8 bytes) stays within this
+constexpr size_t kExactKeysBytes = size_t(512) << 20;
 
 int run_exact(ance_index* ix, const float* Q, const int* qlist, int nq, int k, float* D, int64_t* I,
               int64_t row_offset, cudaStream_t st) {
@@ -830,26 +938,36 @@ int run_exact(ance_index* ix, const float* Q, const int* qlist, int nq, int k, f
   ep.n_rows = ix->n;
   ep.nq_dev = nullptr;
   ep.k = static_cast<int>(std::min<int64_t>(k, std::max<int64_t>(ix->n, 1)));
-  ep.k = std::min(ep.k, 512);
+  ep.k = std::min(ep.k, kMaxK);
   const int sms = gemm::sm_count();
   int n_chunks = static_cast<int>(std::min<int64_t>(2 * sms, (ix->n + 4095) / 4096));
   if (n_chunks < 1) n_chunks = 1;
   ep.n_chunks = n_chunks;
-  const int batch = std::min(nq, kExactBatch);
+  const bool large = ep.k > 512;
+  int batch = std::min(nq, kExactBatch);
+  if (large) {
+    const size_t per_query = static_cast<size_t>(n_chunks) * ep.k * 8;
+    batch = std::min<int>(batch, std::max<int>(kExQB, static_cast<int>(kExactKeysBytes / per_query) / kExQB * kExQB));
+  }
   int rc = ensure(&ix->chunk_keys, &ix->chunk_keys_elems, static_cast<size_t>(batch) * n_chunks * ep.k);
   if (rc) return rc;
   ep.chunk_keys = ix->chunk_keys;
-  const size_t smem = static_cast<size_t>(kExQB) * kExBuf * 8 + static_cast<size_t>(kExQB) * ix->dim * 4;
+  const int buf = large ? kExBufLarge : kExBufSmall;
+  const size_t smem = static_cast<size_t>(kExQB) * buf * 8 + static_cast<size_t>(kExQB) * ix->dim * 4;
   // per device and cheap: set on every call rather than behind a process-wide flag
-  ANCE_CUDA(cudaFuncSetAttribute(exact_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-  for (int b0 = 0; b0 < nq; b0 += kExactBatch) {
-    const int nb = std::min(kExactBatch, nq - b0);
+  if (large)
+    ANCE_CUDA(cudaFuncSetAttribute(exact_chunk_kernel<kExBufLarge>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  else
+    ANCE_CUDA(cudaFuncSetAttribute(exact_chunk_kernel<kExBufSmall>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+  for (int b0 = 0; b0 < nq; b0 += batch) {
+    const int nb = std::min(batch, nq - b0);
     ep.qlist = qlist ? qlist + b0 : nullptr;
     ep.q_base = b0;
     ep.nq = nb;
     const int gy = std::max(1, std::min((nb + kExQB - 1) / kExQB, 128));
     ance::ProfScope ps(ance::kClsExact, st);
-    exact_chunk_kernel<<<dim3(n_chunks, gy), 256, smem, st>>>(ep);
+    if (large) exact_chunk_kernel<kExBufLarge><<<dim3(n_chunks, gy), 256, smem, st>>>(ep);
+    else exact_chunk_kernel<kExBufSmall><<<dim3(n_chunks, gy), 256, smem, st>>>(ep);
     ANCE_CUDA(cudaGetLastError());
     exact_merge_kernel<<<std::max(1, std::min(nb, 4 * sms)), 256, 0, st>>>(ep, D, I, k, row_offset);
     ANCE_CUDA(cudaGetLastError());
@@ -868,7 +986,9 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
                         int64_t row_offset, int* flagged_out, float* flagged_thr_out, int flag_slot, int* ns_out,
                         cudaStream_t st) {
   int rc;
-  const int cap = (kprime <= 512) ? 1024 : 2048;
+  const int cap = (kprime <= 512) ? 1024 : (kprime <= 992) ? 2048 : kWideCap;
+  // candidates per query that rescore_kernel sorts in shared memory
+  const int max_keys = (cap == kWideCap) ? kWideSortKeys : 4096;
   // tier 2 keeps whatever the reservoir holds at the end (at most cap - 32 entries: a fuller one is compacted at once)
   const int out_cap = thr_init ? cap : kprime;
   const int cg = ix->cta_group;
@@ -880,7 +1000,7 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
     // split count whose work-item count fills whole waves best (ties: fewer splits = fewer candidates).
     n_splits = 1;
     if (q_tiles < 2 * clusters) {
-      const int max_splits = std::max(1, std::min(16, 4096 / out_cap));
+      const int max_splits = std::max(1, std::min(16, max_keys / out_cap));
       double best = -1.0;
       for (int sp = 1; sp <= max_splits; ++sp) {
         const long items = static_cast<long>(q_tiles) * sp;
@@ -890,14 +1010,19 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
       }
     }
   }
-  while (n_splits > 1 && n_splits * out_cap > 4096) --n_splits;
-  ANCE_REQUIRE(n_splits * out_cap <= 4096, "ance_index_search: n_splits * candidates per split = %d exceeds 4096", n_splits * out_cap);
+  while (n_splits > 1 && n_splits * out_cap > max_keys) --n_splits;
+  ANCE_REQUIRE(n_splits * out_cap <= max_keys, "ance_index_search: n_splits * candidates per split = %d exceeds %d",
+               n_splits * out_cap, max_keys);
   int ns = 0;
   const bool bf = ix->fmt == ANCE_FMT_BF16;
 #define ANCE_COARSE(CG_, CAP_)                                                                                              \
   rc = bf ? launch_coarse<128, 4, CG_, CAP_, tc05::kFmtBF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st) \
           : launch_coarse<128, 4, CG_, CAP_, tc05::kFmtF16>(ix, Q16, nq, kprime, out_cap, thr_init, n_splits, &ns, st)
-  if (cg == 1 && cap == 1024) { ANCE_COARSE(1, 1024); }
+  if (cap == kWideCap) {
+    if (cg == 1) { ANCE_COARSE(1, kWideCap); }
+    else { ANCE_COARSE(2, kWideCap); }
+  }
+  else if (cg == 1 && cap == 1024) { ANCE_COARSE(1, 1024); }
   else if (cg == 1) { ANCE_COARSE(1, 2048); }
   else if (cap == 1024) { ANCE_COARSE(2, 1024); }
   else { ANCE_COARSE(2, 2048); }
@@ -1019,6 +1144,86 @@ int prepare_operands(ance_index* ix, cudaStream_t st) {
   return ANCE_OK;
 }
 
+// Tiers 1-3 of one search over queries q_dev[0, nq) into D / I [nq, k]; the counts are added to *acc (nq, kprime and
+// the stream are the caller's).  tier2_kprime: what tier 2 compacts an overflowing reservoir to (>= k).
+int search_tiers(ance_index* ix, const float* q_dev, int64_t nq, int k, int kprime, int tier2_kprime, float* D_dev,
+                 int64_t* I_dev, int64_t row_offset, cudaStream_t st, ance_search_stats* acc) {
+  int rc;
+  // --- 1. quantize queries
+  {
+    size_t a = static_cast<size_t>(ix->q_cap) * ix->dim, b = ix->q_cap, c = ix->q_cap;
+    if ((rc = ensure(&ix->Q16, &a, static_cast<size_t>(nq) * ix->dim))) return rc;
+    if ((rc = ensure(&ix->qn_hat, &b, static_cast<size_t>(nq)))) return rc;
+    if ((rc = ensure(&ix->qn_delta, &c, static_cast<size_t>(nq)))) return rc;
+    ix->q_cap = std::max<int64_t>(ix->q_cap, nq);
+    size_t f = ix->flagged_cap, g = ix->flagged_cap;
+    if ((rc = ensure(&ix->flagged, &f, static_cast<size_t>(nq)))) return rc;
+    if ((rc = ensure(&ix->flagged_thr, &g, static_cast<size_t>(nq)))) return rc;
+    ix->flagged_cap = f;
+  }
+  ANCE_CUDA(cudaMemsetAsync(ix->counters, 0, kCntRowErr * sizeof(int), st));   // everything but the sticky row flag
+  const unsigned qblocks = static_cast<unsigned>((nq + 7) / 8);
+  ance::prof_begin(ance::kClsQuant, st);
+  if (ix->fmt == ANCE_FMT_BF16)
+    quantize_rows_kernel<true><<<qblocks, 256, 0, st>>>(q_dev, ix->Q16, nq, ix->dim, nullptr, ix->qn_hat, ix->qn_delta, nullptr, ix->counters + kCntQueryErr);
+  else
+    quantize_rows_kernel<false><<<qblocks, 256, 0, st>>>(q_dev, ix->Q16, nq, ix->dim, nullptr, ix->qn_hat, ix->qn_delta, nullptr, ix->counters + kCntQueryErr);
+  ance::prof_end(ance::kClsQuant, st);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  // --- 2+3. tier 1: coarse pass over all queries, exact rescoring, certificate
+  int ns = 0;
+  rc = coarse_rescore_pass(ix, ix->Q16, q_dev, nq, nullptr, kprime, nullptr, ix->n_splits, k, D_dev, I_dev, row_offset,
+                           ix->flagged, ix->flagged_thr, 0, &ns, st);
+  if (rc) return rc;
+  // One small D2H + sync per search tells the host how many queries stay uncertified and whether an operand left
+  // the 16-bit format's range (the reference's search call is synchronous as well).
+  int h[kNumCounters] = {};
+  ANCE_CUDA(cudaMemcpyAsync(h, ix->counters, sizeof(h), cudaMemcpyDeviceToHost, st));
+  ANCE_CUDA(cudaStreamSynchronize(st));
+  if (h[kCntQueryErr] || h[kCntRowErr]) {
+    // coarse scores, thresholds and the certificate would be compared against inf / NaN: refuse instead of
+    // returning ANCE_OK with unverifiable neighbours
+    ance::set_error("ance_index_search: %s non-finite after rounding to %s (inf / NaN in the input%s)",
+                    h[kCntRowErr] ? "an index row is" : "a query is", ix->fmt == ANCE_FMT_FP16 ? "fp16" : "bf16",
+                    ix->fmt == ANCE_FMT_FP16 ? ", or |x| > 65504: switch with ance_index_set_param(\"operand_fmt\", ANCE_FMT_BF16)" : "");
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  int n_exact = h[0];
+  int ns2 = 0;
+  if (h[0] > 0 && ix->tier2 && ix->n >= 4 * static_cast<int64_t>(tier2_kprime)) {
+    // --- tier 2: the uncertified queries once more, from their own thresholds (nothing that passes is dropped)
+    const int n2 = h[0];
+    if ((rc = ensure(&ix->Q16b, &ix->q16b_elems, static_cast<size_t>(n2) * ix->dim))) return rc;
+    if ((rc = ensure(&ix->flagged2, &ix->flagged2_cap, static_cast<size_t>(n2)))) return rc;
+    gather_rows16_kernel<<<n2, 96, 0, st>>>(ix->Q16, ix->flagged, n2, ix->dim, ix->Q16b);
+    ANCE_CUDA(cudaGetLastError());
+    ance::count_launch(1);
+    rc = coarse_rescore_pass(ix, ix->Q16b, q_dev, n2, ix->flagged, tier2_kprime, ix->flagged_thr, 0, k, D_dev, I_dev, row_offset,
+                             ix->flagged2, nullptr, 3, &ns2, st);
+    if (rc) return rc;
+    ANCE_CUDA(cudaMemcpyAsync(h, ix->counters, sizeof(h), cudaMemcpyDeviceToHost, st));
+    ANCE_CUDA(cudaStreamSynchronize(st));
+    n_exact = h[3];
+    if (n_exact > 0 && ix->exact_fallback) {
+      rc = run_exact(ix, q_dev, ix->flagged2, n_exact, k, D_dev, I_dev, row_offset, st);
+      if (rc) return rc;
+    }
+  } else if (n_exact > 0 && ix->exact_fallback) {
+    // --- tier 3: exact brute force
+    rc = run_exact(ix, q_dev, ix->flagged, n_exact, k, D_dev, I_dev, row_offset, st);
+    if (rc) return rc;
+  }
+  acc->n_splits = std::max(acc->n_splits, ns);
+  acc->n_tier2 += h[0];
+  acc->n_uncertified += n_exact;
+  acc->n_candidates += h[1];
+  float eps;
+  memcpy(&eps, &h[2], 4);
+  acc->max_eps = std::max(acc->max_eps, eps);
+  return ANCE_OK;
+}
+
 }  // namespace
 
 extern "C" int ance_index_create(int dim, int64_t capacity_rows, int operand_fmt, ance_index_t* out) {
@@ -1082,7 +1287,7 @@ extern "C" int ance_index_prepare(ance_index_t ix, void* stream) {
 extern "C" int ance_index_set_param(ance_index_t ix, const char* name, double value) {
   ANCE_REQUIRE(ix != nullptr && name != nullptr, "ance_index_set_param: null argument");
   const int v = static_cast<int>(value);
-  if (!strcmp(name, "kprime")) { ANCE_REQUIRE(v >= 0 && v <= 1024 && v % 32 == 0, "kprime must be a multiple of 32 in [0, 1024]"); ix->kprime = v; }
+  if (!strcmp(name, "kprime")) { ANCE_REQUIRE(v >= 0 && v <= kWideKPrimeMax && v % 32 == 0, "kprime must be a multiple of 32 in [0, %d]", kWideKPrimeMax); ix->kprime = v; }
   else if (!strcmp(name, "n_splits")) { ANCE_REQUIRE(v >= 0 && v <= 64, "n_splits must be in [0, 64]"); ix->n_splits = v; }
   else if (!strcmp(name, "cta_group")) { ANCE_REQUIRE(v == 1 || v == 2, "cta_group must be 1 or 2"); ix->cta_group = v; }
   else if (!strcmp(name, "exact_fallback")) { ix->exact_fallback = v != 0; }
@@ -1107,7 +1312,7 @@ extern "C" int ance_index_set_param(ance_index_t ix, const char* name, double va
 extern "C" int ance_index_search_exact(ance_index_t ix, const float* q_dev, int64_t nq, int k, float* D_dev,
                                        int64_t* I_dev, int64_t row_offset, void* stream) {
   ANCE_REQUIRE(ix != nullptr, "ance_index_search_exact: null handle");
-  ANCE_REQUIRE(nq >= 0 && k > 0 && k <= 512, "ance_index_search_exact: need nq >= 0 and 0 < k <= 512");
+  ANCE_REQUIRE(nq >= 0 && k > 0 && k <= kMaxK, "ance_index_search_exact: need nq >= 0 and 0 < k <= %d", kMaxK);
   if (nq == 0) return ANCE_OK;
   ANCE_REQUIRE(q_dev && D_dev && I_dev, "ance_index_search_exact: null buffer");
   int rc = check_handle_device(ix, "ance_index_search_exact");
@@ -1138,93 +1343,43 @@ extern "C" int ance_index_search(ance_index_t ix, const float* q_dev, int64_t nq
   // choose k' (candidates kept per split).  The certificate needs every row within eps of the k-th score among the
   // candidates; eps is ~0.5 (fp16 operands) / ~3 (bf16) for rows of norm 27.7, i.e. ~0.1 k / ~0.6 k extra rows on the
   // distributions of tools/exp_certify.py.  A query that k' does not cover costs one tier-2 pass, not a wrong answer.
+  const bool wide = k > 512;   // the large-k path (kWideCap reservoirs, query blocks)
   int kprime = ix->kprime;
   if (kprime == 0) {
     const int want = (ix->fmt == ANCE_FMT_FP16) ? k + k / 2 - k / 16 : 2 * k + 32;   // fp16: ~1.44 k (k = 200: 288)
-    kprime = (k <= 240) ? std::min(512, std::max(64, (want + 31) / 32 * 32)) : std::min(992, (2 * k + 31) / 32 * 32);
+    if (!wide)
+      kprime = (k <= 240) ? std::min(512, std::max(64, (want + 31) / 32 * 32)) : std::min(992, (2 * k + 31) / 32 * 32);
+    else
+      kprime = std::min(kWideKPrimeMax, std::max(kWideKPrimeMin, (want + 31) / 32 * 32));
   }
-  if (kprime < k || kprime > 992 || k > 512 || ix->n < 4 * static_cast<int64_t>(kprime)) {
+  if (kprime < k || kprime > (wide ? kWideKPrimeMax : 992) || k > kMaxK || ix->n < 4 * static_cast<int64_t>(kprime)) {
     // tiny index or very large k: the exact brute-force path is both correct and cheap enough
-    ANCE_REQUIRE(k <= 512, "ance_index_search: k = %d > 512 is not supported", k);
+    ANCE_REQUIRE(k <= kMaxK, "ance_index_search: k = %d > %d is not supported", k, kMaxK);
     ix->stats = ance_search_stats{};
     ix->stats.nq = nq;
     ix->stats.n_uncertified = nq;
     return ance_index_search_exact(ix, q_dev, nq, k, D_dev, I_dev, row_offset, stream);
   }
   if ((rc = prepare_operands(ix, st))) return rc;
-  // --- 1. quantize queries
-  {
-    size_t a = static_cast<size_t>(ix->q_cap) * ix->dim, b = ix->q_cap, c = ix->q_cap;
-    if ((rc = ensure(&ix->Q16, &a, static_cast<size_t>(nq) * ix->dim))) return rc;
-    if ((rc = ensure(&ix->qn_hat, &b, static_cast<size_t>(nq)))) return rc;
-    if ((rc = ensure(&ix->qn_delta, &c, static_cast<size_t>(nq)))) return rc;
-    ix->q_cap = std::max<int64_t>(ix->q_cap, nq);
-    size_t f = ix->flagged_cap, g = ix->flagged_cap;
-    if ((rc = ensure(&ix->flagged, &f, static_cast<size_t>(nq)))) return rc;
-    if ((rc = ensure(&ix->flagged_thr, &g, static_cast<size_t>(nq)))) return rc;
-    ix->flagged_cap = f;
-  }
-  ANCE_CUDA(cudaMemsetAsync(ix->counters, 0, kCntRowErr * sizeof(int), st));   // everything but the sticky row flag
-  const unsigned qblocks = static_cast<unsigned>((nq + 7) / 8);
-  ance::prof_begin(ance::kClsQuant, st);
-  if (ix->fmt == ANCE_FMT_BF16)
-    quantize_rows_kernel<true><<<qblocks, 256, 0, st>>>(q_dev, ix->Q16, nq, ix->dim, nullptr, ix->qn_hat, ix->qn_delta, nullptr, ix->counters + kCntQueryErr);
-  else
-    quantize_rows_kernel<false><<<qblocks, 256, 0, st>>>(q_dev, ix->Q16, nq, ix->dim, nullptr, ix->qn_hat, ix->qn_delta, nullptr, ix->counters + kCntQueryErr);
-  ance::prof_end(ance::kClsQuant, st);
-  ANCE_CUDA(cudaGetLastError());
-  ance::count_launch(1);
-  // --- 2+3. tier 1: coarse pass over all queries, exact rescoring, certificate
-  int ns = 0;
-  rc = coarse_rescore_pass(ix, ix->Q16, q_dev, nq, nullptr, kprime, nullptr, ix->n_splits, k, D_dev, I_dev, row_offset,
-                           ix->flagged, ix->flagged_thr, 0, &ns, st);
-  if (rc) return rc;
-  // One small D2H + sync per search tells the host how many queries stay uncertified and whether an operand left
-  // the 16-bit format's range (the reference's search call is synchronous as well).
-  int h[kNumCounters] = {};
-  ANCE_CUDA(cudaMemcpyAsync(h, ix->counters, sizeof(h), cudaMemcpyDeviceToHost, st));
-  ANCE_CUDA(cudaStreamSynchronize(st));
-  if (h[kCntQueryErr] || h[kCntRowErr]) {
-    // coarse scores, thresholds and the certificate would be compared against inf / NaN: refuse instead of
-    // returning ANCE_OK with unverifiable neighbours
-    ance::set_error("ance_index_search: %s non-finite after rounding to %s (inf / NaN in the input%s)",
-                    h[kCntRowErr] ? "an index row is" : "a query is", ix->fmt == ANCE_FMT_FP16 ? "fp16" : "bf16",
-                    ix->fmt == ANCE_FMT_FP16 ? ", or |x| > 65504: switch with ance_index_set_param(\"operand_fmt\", ANCE_FMT_BF16)" : "");
-    return ANCE_ERR_UNSUPPORTED;
-  }
-  int n_exact = h[0];
-  int ns2 = 0;
-  if (h[0] > 0 && ix->tier2 && ix->n >= 4 * 992) {
-    // --- tier 2: the uncertified queries once more, from their own thresholds (nothing that passes is dropped)
-    const int n2 = h[0];
-    if ((rc = ensure(&ix->Q16b, &ix->q16b_elems, static_cast<size_t>(n2) * ix->dim))) return rc;
-    if ((rc = ensure(&ix->flagged2, &ix->flagged2_cap, static_cast<size_t>(n2)))) return rc;
-    gather_rows16_kernel<<<n2, 96, 0, st>>>(ix->Q16, ix->flagged, n2, ix->dim, ix->Q16b);
-    ANCE_CUDA(cudaGetLastError());
-    ance::count_launch(1);
-    rc = coarse_rescore_pass(ix, ix->Q16b, q_dev, n2, ix->flagged, 992, ix->flagged_thr, 0, k, D_dev, I_dev, row_offset,
-                             ix->flagged2, nullptr, 3, &ns2, st);
+  ance_search_stats acc{};
+  if (!wide) {
+    rc = search_tiers(ix, q_dev, nq, k, kprime, 992, D_dev, I_dev, row_offset, st, &acc);
     if (rc) return rc;
-    ANCE_CUDA(cudaMemcpyAsync(h, ix->counters, sizeof(h), cudaMemcpyDeviceToHost, st));
-    ANCE_CUDA(cudaStreamSynchronize(st));
-    n_exact = h[3];
-    if (n_exact > 0 && ix->exact_fallback) {
-      rc = run_exact(ix, q_dev, ix->flagged2, n_exact, k, D_dev, I_dev, row_offset, st);
+  } else {
+    // Equal blocks of at most kWideQBlock queries (a multiple of the 256-query tile), all tiers per block: the query
+    // copies, candidate lists and flagged lists are sized by the block, not by nq.  Tier 2 compacts to kWideKPrimeMax.
+    const int64_t n_blocks = (nq + kWideQBlock - 1) / kWideQBlock;
+    const int64_t qb = std::min<int64_t>(kWideQBlock, ((nq + n_blocks - 1) / n_blocks + 255) / 256 * 256);
+    for (int64_t b0 = 0; b0 < nq; b0 += qb) {
+      const int64_t nb = std::min(qb, nq - b0);
+      rc = search_tiers(ix, q_dev + b0 * ix->dim, nb, k, kprime, kWideKPrimeMax, D_dev + b0 * k, I_dev + b0 * k,
+                        row_offset, st, &acc);
       if (rc) return rc;
     }
-  } else if (n_exact > 0 && ix->exact_fallback) {
-    // --- tier 3: exact brute force
-    rc = run_exact(ix, q_dev, ix->flagged, n_exact, k, D_dev, I_dev, row_offset, st);
-    if (rc) return rc;
   }
-  ix->stats = ance_search_stats{};
-  ix->stats.nq = nq;
-  ix->stats.kprime = kprime;
-  ix->stats.n_splits = ns;
-  ix->stats.n_tier2 = h[0];
-  ix->stats.n_uncertified = n_exact;
-  ix->stats.n_candidates = h[1];
-  memcpy(&ix->stats.max_eps, &h[2], 4);
+  acc.nq = nq;
+  acc.kprime = kprime;
+  ix->stats = acc;
   ix->last_stream = st;
   return ANCE_OK;
 }

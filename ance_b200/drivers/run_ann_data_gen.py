@@ -560,6 +560,17 @@ def generate_new_ann(args, output_num, checkpoint_path, training_query_positive_
 # =============================================================================================
 # CLI (flags of run_ann_data_gen.py:443-627, plus three GPU knobs at the end)
 # =============================================================================================
+MAX_TOPK = 2048   # largest k ance_index_search serves
+
+
+def topk_arg(v: str) -> int:
+    """--topk_training: checked while parsing, since the search would refuse it only after the whole corpus is encoded."""
+    k = int(v)
+    if not 0 < k <= MAX_TOPK:
+        raise argparse.ArgumentTypeError(f"must be in [1, {MAX_TOPK}], got {k}")
+    return k
+
+
 def get_arguments(argv=None):
     p = argparse.ArgumentParser()
     p.add_argument("--data_dir", default=None, type=str, required=True)
@@ -576,7 +587,7 @@ def get_arguments(argv=None):
     p.add_argument("--max_doc_character", default=10000, type=int)
     p.add_argument("--per_gpu_eval_batch_size", default=128, type=int)
     p.add_argument("--ann_chunk_factor", default=5, type=int)
-    p.add_argument("--topk_training", default=500, type=int)
+    p.add_argument("--topk_training", default=500, type=topk_arg)
     p.add_argument("--negative_sample", default=5, type=int)
     p.add_argument("--ann_measure_topk_mrr", default=False, action="store_true")
     p.add_argument("--only_keep_latest_embedding_file", default=False, action="store_true")

@@ -132,7 +132,10 @@ class IndexFlatIP:
     # -- search ------------------------------------------------------------------------------------
     def search_device(self, q: torch.Tensor, k: int, row_offset: int = 0, exact: bool = False
                       ) -> Tuple[torch.Tensor, torch.Tensor]:
-        """Q [nq, d] fp32 CUDA -> (D [nq, k] fp32, I [nq, k] int64), both CUDA, stream-ordered."""
+        """Q [nq, d] fp32 CUDA -> (D [nq, k] fp32, I [nq, k] int64), both CUDA, stream-ordered.  0 < k <= 2048 (faiss's
+        GPU limit; top-1000 full-rank evaluation needs k = 1000), else AnceError.  k > 512 runs the large-k path: wider
+        reservoirs, queries in blocks of at most 16,384 (workspace about 2.2 GB whatever nq is).  exact: every query by
+        the fp64 brute-force kernel (the validation path)."""
         nq = int(q.shape[0])
         D = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
@@ -158,7 +161,7 @@ class IndexFlatIP:
 
     def search(self, x, k: int):
         """IndexFlatIP.search: returns (D, I) as numpy arrays for numpy input (the reference's
-        usage) or CUDA tensors for CUDA input."""
+        usage) or CUDA tensors for CUDA input.  0 < k <= 2048; with fewer than k rows the tail is -1 / lowest float."""
         was_numpy = isinstance(x, np.ndarray)
         if x.shape[1] != self.d:
             raise ValueError(f"dimension mismatch: index {self.d}, queries {x.shape[1]}")

@@ -76,15 +76,22 @@ int ance_index_add(ance_index_t idx, const float* rows_dev, int64_t n, void* str
  * norms) and rounded to operand_fmt.  ance_index_search does this itself when rows were added since the last time
  * (8.84M rows: ~10 ms); call it explicitly to keep that cost out of the first search. */
 int ance_index_prepare(ance_index_t idx, void* stream);
-/* IndexFlatIP.search: Q [nq, dim] fp32 -> D [nq, k] fp32, I [nq, k] int64 (all device memory). */
+/* IndexFlatIP.search: Q [nq, dim] fp32 -> D [nq, k] fp32, I [nq, k] int64 (all device memory), 0 < k <= 2048
+ * (ANCE_ERR_INVALID above).  k <= 512: reservoirs of 1024 / 2048 entries, k' <= 992.  512 < k <= 2048 (top-1000
+ * evaluation, large --topk_training): reservoirs of 8192 entries, k' in [1024, 4096], queries processed in blocks of at
+ * most 16,384 so that the workspace does not grow with nq; at k = 1000 and k = 2048 alike it peaks at about 2.2 GB on a
+ * 132-SM H100 (reservoirs 1.11 GB, candidate ids <= 0.54 GB, brute-force keys <= 0.54 GB, query copies 0.05 GB), on top
+ * of the index's own 6 bytes per row element. */
 int ance_index_search(ance_index_t idx, const float* q_dev, int64_t nq, int k, float* D_dev, int64_t* I_dev,
                       int64_t row_offset, void* stream);
-/* Same contract, computed entirely by the exact fp32->fp64 brute-force kernel (validation path). */
+/* Same contract (0 < k <= 2048), computed entirely by the exact fp32->fp64 brute-force kernel (validation path). */
 int ance_index_search_exact(ance_index_t idx, const float* q_dev, int64_t nq, int k, float* D_dev,
                             int64_t* I_dev, int64_t row_offset, void* stream);
 /* Statistics of the last search (ance_index_search has already synchronised its stream). */
 int ance_index_last_stats(ance_index_t idx, ance_search_stats* out);
-/* Tunables: "kprime" (0 = auto: about 1.44 k for fp16 operands, 2 k for bf16), "n_splits" (0 = auto), "cta_group" (1|2),
+/* Tunables: "kprime" (multiple of 32 in [0, 4096]; 0 = auto: about 1.44 k for fp16 operands, 2 k + 32 for bf16, at least
+ * 1024 when k > 512; a value below k, or above 992 when k <= 512, sends the search to the brute force), "n_splits"
+ * (0 = auto), "cta_group" (1|2),
  * "max_ctas" (0 = all SMs), "tier2" (0|1), "exact_fallback" (0|1: measurement only — results of uncertified queries are
  * then NOT guaranteed), "pace_window" (tiles a sweeping CTA pair may run ahead of the slowest one; 0 = no soft
  * barrier), "operand_fmt" (ANCE_FMT_*: the rows already added are re-rounded from the fp32 copy at the next prepare / search),
