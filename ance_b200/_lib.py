@@ -61,6 +61,10 @@ SIGNATURES = {
     "ance_launch_count": (C.c_int64, []),
     "ance_index_create": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_void_p)]),
     "ance_index_create_over": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ance_index_create_host": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ance_index_memory": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "ance_index_last_fetched": (C.c_int64, [C.c_void_p]),
+    "ance_index_host_rows": (C.c_void_p, [C.c_void_p]),
     "ance_index_destroy": (C.c_int, [C.c_void_p]),
     "ance_index_reset": (C.c_int, [C.c_void_p]),
     "ance_index_ntotal": (C.c_int64, [C.c_void_p]),

@@ -405,22 +405,46 @@ struct EpTopK {
 // ------------------------------------------------------------------------------------------------
 // shared helpers: exact dot products and block bitonic sort
 // ------------------------------------------------------------------------------------------------
+// Loads of fp32 index rows.  kHost: the rows are pinned host memory mapped into the device's address space (a host
+// index): plain ld.global, never the non-coherent read-only path.  Otherwise __ldg, as the device index always had.
+template <bool kHost>
+__device__ __forceinline__ float4 ld_rows4(const float* p) {
+  if constexpr (kHost) {
+    float4 v;
+    asm("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+    return v;
+  } else {
+    return __ldg(reinterpret_cast<const float4*>(p));
+  }
+}
+template <bool kHost>
+__device__ __forceinline__ float ld_rows1(const float* p) {
+  if constexpr (kHost) {
+    float v;
+    asm("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p));
+    return v;
+  } else {
+    return __ldg(p);
+  }
+}
+
 // exact <q, p>: fp32 inputs, products and sum in fp64 (each product is exact in fp64), result
 // rounded once to fp32.  Lane-strided float4 loads; deterministic shuffle tree.
+template <bool kHost = false>
 __device__ __forceinline__ double warp_dot_f64(const float* __restrict__ q_smem, const float* __restrict__ p, int d,
                                                int lane) {
   double acc = 0.0;
   if ((d & 127) == 0) {
     for (int i = lane * 4; i < d; i += 128) {
       const float4 a = *reinterpret_cast<const float4*>(q_smem + i);
-      const float4 b = __ldg(reinterpret_cast<const float4*>(p + i));
+      const float4 b = ld_rows4<kHost>(p + i);
       acc = fma(static_cast<double>(a.x), static_cast<double>(b.x), acc);
       acc = fma(static_cast<double>(a.y), static_cast<double>(b.y), acc);
       acc = fma(static_cast<double>(a.z), static_cast<double>(b.z), acc);
       acc = fma(static_cast<double>(a.w), static_cast<double>(b.w), acc);
     }
   } else {
-    for (int i = lane; i < d; i += 32) acc = fma(static_cast<double>(q_smem[i]), static_cast<double>(__ldg(p + i)), acc);
+    for (int i = lane; i < d; i += 32) acc = fma(static_cast<double>(q_smem[i]), static_cast<double>(ld_rows1<kHost>(p + i)), acc);
   }
 #pragma unroll
   for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
@@ -479,12 +503,18 @@ struct RescoreParams {
   int* counters;       // [0] tier-1 flagged [1] n_candidates [2] max eps bits [3] tier-2 flagged
   unsigned int* max_eps;
   int sort_n;          // pow2 >= total candidates of a query
+  // host index only (rescore_kernel<true>): the pre-filter's inputs
+  const uint16_t* P16;      // [n, d] 16-bit operand rows (centred, rounded)
+  const float* ndelta;      // [n] ||p_j - mu - p^_j|| per row, rounded up
+  int bf16;                 // operand format of P16
 };
+
+constexpr int kCntFetched = 4;   // counters[4]: rows rescoring read from host memory (host index)
 
 // exact <q, p_c> of kNB candidate rows at once: all the row's 16-byte loads (d / 128 per lane and row) are issued
 // before the first fp64 FMA, so a warp keeps kNB * d / 128 gathers in flight instead of one (the rows are random
 // 3 KB reads: latency, not bandwidth, bounded the one-row-at-a-time form at 0.14 of HBM).  kJ = d / 128 (768: kJ = 6).
-template <int kNB, int kJ>
+template <int kNB, int kJ, bool kHost = false>
 __device__ __forceinline__ void warp_dots_f64(const float* __restrict__ q_smem, const float* const (&rows)[kNB], int d,
                                               int lane, double (&out)[kNB]) {
   float4 b[kNB][kJ];
@@ -492,7 +522,7 @@ __device__ __forceinline__ void warp_dots_f64(const float* __restrict__ q_smem, 
   for (int j = 0; j < kJ; ++j) {
     {
 #pragma unroll
-      for (int c = 0; c < kNB; ++c) b[c][j] = __ldg(reinterpret_cast<const float4*>(rows[c] + j * 128 + lane * 4));
+      for (int c = 0; c < kNB; ++c) b[c][j] = ld_rows4<kHost>(rows[c] + j * 128 + lane * 4);
     }
   }
 #pragma unroll
@@ -517,6 +547,151 @@ __device__ __forceinline__ void warp_dots_f64(const float* __restrict__ q_smem, 
   }
 }
 
+// order-preserving double -> uint64 (larger double -> larger key; every non-NaN value maps above 0)
+__device__ __forceinline__ uint64_t d2ord(double x) {
+  const uint64_t u = static_cast<uint64_t>(__double_as_longlong(x));
+  return u ^ (static_cast<uint64_t>(static_cast<int64_t>(u) >> 63) | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double ord2d(uint64_t k) {
+  return __longlong_as_double(static_cast<long long>((k & 0x8000000000000000ull) ? (k ^ 0x8000000000000000ull) : ~k));
+}
+
+// Candidate scores of a HOST index (rows in pinned host memory, every fp32 row read crosses PCIe): a pre-filter on data
+// in HBM, then exact scores of the survivors only.  Writes keys[pos] of every candidate position (0 for a pruned one).
+//   Phase A: s~_j = <q, p^_j> in fp64 from the 16-bit operand row (the products are exact in fp64), and
+//            lo_j / hi_j = <q, mu> + s~_j -/+ (||q|| ||delta_j|| + g), so lo_j <= <q, p_j> <= hi_j; g bounds the fp64
+//            summation error of one dot product over d terms, (d + 16) 2^-53 ||q|| ||p||, for every row (DESIGN.md §4.2).
+//            L = k-th largest lo.
+//   Phase B: prune j iff fl32_up(hi_j + g) < fl32_down(L - g), and compute the exact score of every other candidate
+//            (the same warp_dots_f64 association as the device index: bit-identical scores).
+// At least k candidates score >= fl32_down(L - g) and a pruned row scores <= fl32_up(hi_j + g), strictly less: the top k
+// of the survivors are the top k of all candidates, ties included, and the certificate sees the same k-th score.
+// extra: 16 * sort_n bytes of shared memory (hi [sort_n] fp64, rows [sort_n], survivors [sort_n]).
+__device__ __forceinline__ void host_rows_scores(const RescoreParams& p, uint64_t* keys, const float* qs, const int* offs,
+                                              const double* s_qmu, uint8_t* extra, int ql) {
+  double* hi = reinterpret_cast<double*>(extra);
+  int* rows = reinterpret_cast<int*>(hi + p.sort_n);
+  int* surv = rows + p.sort_n;
+  __shared__ double s_red[2][8];
+  __shared__ double s_g;
+  __shared__ double s_qn;
+  __shared__ double s_base;
+  __shared__ float s_T;
+  __shared__ int s_nsurv;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int d = p.d, m = offs[p.n_splits];
+  double qq = 0.0, mm = 0.0;
+  for (int i = threadIdx.x; i < d; i += blockDim.x) {
+    qq = fma(static_cast<double>(qs[i]), static_cast<double>(qs[i]), qq);
+    if (p.mu) mm = fma(static_cast<double>(__ldg(p.mu + i)), static_cast<double>(__ldg(p.mu + i)), mm);
+  }
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    qq += __shfl_xor_sync(0xffffffffu, qq, s);
+    mm += __shfl_xor_sync(0xffffffffu, mm, s);
+  }
+  if (lane == 0) {
+    s_red[0][warp] = qq;
+    s_red[1][warp] = mm;
+  }
+  for (int s = 0; s < p.n_splits; ++s) {
+    const int* ids = p.cand_id + (static_cast<size_t>(ql) * p.n_splits + s) * p.cand_stride;
+    for (int c = threadIdx.x; c < offs[s + 1] - offs[s]; c += blockDim.x) rows[offs[s] + c] = ids[c];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sq = 0.0, sm = 0.0, qmu = 0.0;
+    for (int w = 0; w < nwarps; ++w) {
+      sq += s_red[0][w];
+      sm += s_red[1][w];
+      qmu += s_qmu[w];
+    }
+    // every fp64 sum of d products above carries a relative error below (d + 16) 2^-53: inflate by twice that
+    const double infl = 1.0 + static_cast<double>(d + 16) * 0x1p-52;
+    const double qn = __dsqrt_ru(__dmul_ru(sq, infl));
+    const double mun = __dsqrt_ru(__dmul_ru(sm, infl));
+    const double maxp = static_cast<double>(__uint_as_float(p.pstats[0])), maxdp = static_cast<double>(__uint_as_float(p.pstats[1]));
+    // g >= (d + 16) 2^-53 ||q|| ||x|| with ||x|| <= ||mu|| + max ||p^|| + max ||delta||: covers the summation error of
+    // s~_j + <q, mu> (one g) and of the exact fp64 score (the other g)
+    s_g = __dmul_ru(__dmul_ru(static_cast<double>(d + 16) * 0x1p-53, qn), __dadd_ru(__dadd_ru(mun, maxp), maxdp));
+    s_qn = qn;
+    s_base = qmu;
+  }
+  __syncthreads();
+  const double g = s_g, qn = s_qn, qmu = s_base;
+  // ||delta_j|| is an fp32 sum of d squares (+ sqrt): charge its relative rounding error once more
+  const double nd_infl = 1.0 + static_cast<double>(d + 64) * 0x1p-23;
+  // --- phase A: bounds from the 16-bit rows in HBM
+  for (int c = warp; c < m; c += nwarps) {
+    const int row = rows[c];
+    const uint16_t* r16 = p.P16 + static_cast<size_t>(row) * d;
+    double acc = 0.0;
+    for (int i = lane * 8; i < d; i += 256) {   // d % 8 == 0 (checked at creation)
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(r16 + i));
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      // the lane's 8 query values as two 16-byte shared loads (a warp reads 1 KB contiguously: no bank conflicts)
+      const float4 qa = *reinterpret_cast<const float4*>(qs + i), qb = *reinterpret_cast<const float4*>(qs + i + 4);
+      const float qv[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const uint16_t h = static_cast<uint16_t>(w[t >> 1] >> ((t & 1) * 16));
+        const float x = p.bf16 ? __uint_as_float(static_cast<uint32_t>(h) << 16) : __half2float(__ushort_as_half(h));
+        acc = fma(static_cast<double>(qv[t]), static_cast<double>(x), acc);
+      }
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
+    if (lane == 0) {
+      const double r = __dadd_ru(__dmul_ru(qn, __dmul_ru(static_cast<double>(__ldg(p.ndelta + row)), nd_infl)), g);
+      keys[c] = d2ord(__dadd_rd(__dadd_rd(qmu, acc), -r));
+      hi[c] = __dadd_ru(__dadd_ru(qmu, acc), r);
+    }
+  }
+  // L = k-th largest lo (keys past m stay 0: below every lo)
+  if (m > p.k) {
+    block_bitonic_desc(keys, p.sort_n);
+    if (threadIdx.x == 0) s_T = __double2float_rd(__dadd_rd(ord2d(keys[p.k - 1]), -g));
+  } else if (threadIdx.x == 0) {
+    s_T = -INFINITY;   // at most k candidates: nothing may be pruned
+  }
+  if (threadIdx.x == 0) s_nsurv = 0;
+  __syncthreads();
+  const float T = s_T;
+  for (int c = threadIdx.x; c < m; c += blockDim.x)
+    if (T == -INFINITY || __double2float_ru(__dadd_ru(hi[c], g)) >= T) surv[atomicAdd(&s_nsurv, 1)] = c;
+  for (int i = threadIdx.x; i < p.sort_n; i += blockDim.x) keys[i] = 0ull;
+  __syncthreads();
+  // --- phase B: exact scores of the survivors, fp32 rows read through the mapped host pointer
+  const int ns = s_nsurv;
+  constexpr int kNB = 4;
+  if (d == 768) {
+    for (int c0 = warp * kNB; c0 < ns; c0 += nwarps * kNB) {
+      int pos[kNB];
+      const float* rp[kNB];
+#pragma unroll
+      for (int c = 0; c < kNB; ++c) {
+        pos[c] = surv[min(c0 + c, ns - 1)];
+        rp[c] = p.P + static_cast<size_t>(rows[pos[c]]) * d;
+      }
+      double dot[kNB];
+      warp_dots_f64<kNB, 6, true>(qs, rp, d, lane, dot);
+      if (lane == 0) {
+#pragma unroll
+        for (int c = 0; c < kNB; ++c)
+          if (c0 + c < ns) keys[pos[c]] = make_key(static_cast<float>(dot[c]), static_cast<uint32_t>(rows[pos[c]]));
+      }
+    }
+  } else {
+    for (int c = warp; c < ns; c += nwarps) {
+      const int pos = surv[c];
+      const double dot = warp_dot_f64<true>(qs, p.P + static_cast<size_t>(rows[pos]) * d, d, lane);
+      if (lane == 0) keys[pos] = make_key(static_cast<float>(dot), static_cast<uint32_t>(rows[pos]));
+    }
+  }
+  if (threadIdx.x == 0) atomicAdd(&p.counters[kCntFetched], ns);
+}
+
+template <bool kHost>
 __global__ void __launch_bounds__(256) rescore_kernel(const RescoreParams p) {
   extern __shared__ __align__(16) uint8_t rs_smem[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(rs_smem);
@@ -551,6 +726,10 @@ __global__ void __launch_bounds__(256) rescore_kernel(const RescoreParams p) {
   __syncthreads();
   constexpr int kNB = 4;
   const bool wide = p.d == 768;   // the path's dimension (models.py:145-146); other dims take the one-row loop
+  if constexpr (kHost) {
+    const size_t extra = (static_cast<size_t>(p.sort_n) * 8 + static_cast<size_t>(p.d) * 4 + (p.n_splits + 1) * 4 + 15) & ~size_t(15);
+    host_rows_scores(p, keys, qs, offs, s_qmu, rs_smem + extra, ql);
+  } else
   for (int s = 0; s < p.n_splits; ++s) {
     const int n = offs[s + 1] - offs[s];
     const int* ids = p.cand_id + (static_cast<size_t>(ql) * p.n_splits + s) * p.cand_stride;
@@ -638,11 +817,14 @@ struct ExactParams {
   int nq;
   int k;                 // <= 2048
   int n_chunks;
-  uint64_t* chunk_keys;  // [nq_cap * n_chunks * k]
+  uint64_t* chunk_keys;  // [nq_cap * n_chunks * k]  (run_exact_host: [nq_cap * (n_chunks + 1) * k])
 };
 
-template <int kExBuf>
-__global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
+// kSlab: p.P is a slab of a host index's rows staged in device memory (run_exact_host): keys carry the global row
+// row_base + row, and every query has n_chunks + 1 key slots, the last one holding the best k of the earlier slabs.
+// (row_base is a kernel argument rather than an ExactParams field, which exact_merge_kernel shares.)
+template <int kExBuf, bool kSlab>
+__global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p, int64_t row_base) {
   extern __shared__ __align__(16) uint8_t ex_smem[];
   uint64_t* buf = reinterpret_cast<uint64_t*>(ex_smem);              // [kExQB][kExBuf]
   float* qs = reinterpret_cast<float*>(buf + kExQB * kExBuf);        // [kExQB][d]
@@ -694,7 +876,7 @@ __global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
 #pragma unroll
           for (int qi = 1; qi < kExQB; ++qi)
             if (lane == qi) a = acc[qi];
-          const uint64_t key = make_key(static_cast<float>(a), static_cast<uint32_t>(row));
+          const uint64_t key = make_key(static_cast<float>(a), static_cast<uint32_t>(kSlab ? row_base + row : row));
           if (key > thr[lane]) {
             const int slot = atomicAdd(&cnt[lane], 1);
             buf[lane * kExBuf + slot] = key;  // slot < kExBuf: at most nwarps*kExRound appends per round
@@ -720,7 +902,7 @@ __global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
       const int n = cnt[qi];
       for (int i = n + threadIdx.x; i < kExBuf; i += blockDim.x) buf[qi * kExBuf + i] = 0ull;
       block_bitonic_desc(buf + qi * kExBuf, kExBuf);
-      uint64_t* out = p.chunk_keys + (static_cast<size_t>(g * kExQB + qi) * p.n_chunks + blockIdx.x) * p.k;
+      uint64_t* out = p.chunk_keys + (static_cast<size_t>(g * kExQB + qi) * (kSlab ? p.n_chunks + 1 : p.n_chunks) + blockIdx.x) * p.k;
       for (int i = threadIdx.x; i < p.k; i += blockDim.x) out[i] = (i < n) ? buf[qi * kExBuf + i] : 0ull;
     }
   }
@@ -728,6 +910,8 @@ __global__ void __launch_bounds__(256) exact_chunk_kernel(const ExactParams p) {
 
 constexpr int kMergeBuf = 4096;   // > k: every round merges at least kMergeBuf - k new keys into the best k
 
+// kToAcc: write the merged best k back into the query's last key slot (run_exact_host's running result) instead of D / I
+template <bool kToAcc>
 __global__ void __launch_bounds__(256) exact_merge_kernel(const ExactParams p, float* D, int64_t* I, int out_k,
                                                           int64_t row_offset) {
   __shared__ uint64_t keys[kMergeBuf];
@@ -747,11 +931,16 @@ __global__ void __launch_bounds__(256) exact_merge_kernel(const ExactParams p, f
       block_bitonic_desc(keys, kMergeBuf);
       have = p.k;
     }
+    if constexpr (kToAcc) {
+      uint64_t* acc = p.chunk_keys + (static_cast<size_t>(qi) * p.n_chunks + p.n_chunks - 1) * p.k;
+      for (int i = threadIdx.x; i < p.k; i += blockDim.x) acc[i] = keys[i];
+    } else {
     for (int i = threadIdx.x; i < out_k; i += blockDim.x) {
       const uint64_t key = (i < p.k) ? keys[i] : 0ull;
       const bool ok = key != 0ull;
       D[static_cast<size_t>(q) * out_k + i] = ok ? key_score(key) : -FLT_MAX;
       I[static_cast<size_t>(q) * out_k + i] = ok ? row_offset + static_cast<int64_t>(key_row(key)) : -1;
+    }
     }
     __syncthreads();
   }
@@ -777,8 +966,14 @@ struct ance_index {
   int64_t cap = 0, n = 0;
   int fmt = ANCE_FMT_FP16;
   int device = 0;
-  float* P32 = nullptr;      // [cap, dim]
-  bool owns_p32 = true;      // false: caller-owned storage (ance_index_create_over)
+  float* P32 = nullptr;      // [cap, dim]  (host index: the device address of the pinned host rows)
+  bool owns_p32 = true;      // false: caller-owned storage (ance_index_create_over), or a host index
+  // host index (ance_index_create_host): the fp32 rows live in pinned host memory
+  bool host_rows = false;
+  float* P32_host = nullptr;       // [cap, dim] host address of the rows
+  bool owns_host = false;          // allocated by the library (cudaHostAlloc), freed by ance_index_destroy
+  float* ndelta = nullptr;         // [cap] ||p_j - mu - p^_j|| per row (device; the rescoring pre-filter's bound)
+  int64_t last_fetched = 0;        // rows the last search's rescoring read from host memory
   uint16_t* P16 = nullptr;   // [cap, dim]
   unsigned int* pstats = nullptr;  // [2]
   float* mu = nullptr;             // [dim] centre of the rows (see quantize_rows_kernel)
@@ -796,7 +991,8 @@ struct ance_index {
   int* flagged2 = nullptr; size_t flagged2_cap = 0;
   uint16_t* Q16b = nullptr; size_t q16b_elems = 0;
   int* pace = nullptr;              // [kMaxPace] progress counters of the sweeping CTA pairs (soft barrier)
-  // [0] tier-1 flagged  [1] candidates rescored  [2] max eps bits  [3] tier-2 flagged  [4,5] spare
+  // [0] tier-1 flagged  [1] candidates rescored  [2] max eps bits  [3] tier-2 flagged  [4] rows fetched from host memory
+  // [5] spare
   // [6] a QUERY was non-finite after rounding (cleared per search)  [7] an index ROW was (sticky until reset / requantise)
   int* counters = nullptr;
   uint64_t* chunk_keys = nullptr; size_t chunk_keys_elems = 0;
@@ -929,8 +1125,83 @@ constexpr int kExactBatch = 1024;  // queries per brute-force pass (bounds the c
 // k > 512: fewer queries per pass, so that chunk_keys (batch * n_chunks * k * 8 bytes) stays within this
 constexpr size_t kExactKeysBytes = size_t(512) << 20;
 
+// device staging buffer of a host index's prepare and brute force
+constexpr size_t kHostStageBytes = size_t(512) << 20;
+
+// run_exact on a host index: the rows cross PCIe ONCE per batch of queries.  For each batch the rows are copied H2D slab by
+// slab (at most 512 MB) into a staging buffer; the device brute force runs on the slab with global row numbers and keeps
+// its chunk keys next to a per-query slot holding the best k of the earlier slabs, which exact_merge_kernel<true> updates
+// after every slab; after the last slab exact_merge_kernel<false> writes D / I.  The result is the device path's: the
+// same keys (score, then global row) merged by the same kernels.
+int run_exact_host(ance_index* ix, const float* Q, const int* qlist, int nq, int k, float* D, int64_t* I,
+                   int64_t row_offset, cudaStream_t st) {
+  const int d = ix->dim;
+  const int64_t n = ix->n;
+  const int64_t slab = std::min<int64_t>(n, std::max<int64_t>(1, static_cast<int64_t>(kHostStageBytes / (static_cast<size_t>(d) * 4))));
+  ExactParams ep;
+  ep.Q = Q;
+  ep.d = d;
+  ep.nq_dev = nullptr;
+  ep.k = static_cast<int>(std::min<int64_t>(std::min<int64_t>(k, std::max<int64_t>(n, 1)), kMaxK));
+  const int sms = gemm::sm_count();
+  const int n_chunks = std::max(1, static_cast<int>(std::min<int64_t>(2 * sms, (slab + 4095) / 4096)));
+  ep.n_chunks = n_chunks;
+  const bool large = ep.k > 512;
+  const size_t per_query = static_cast<size_t>(n_chunks + 1) * ep.k * 8;
+  int batch = std::min(nq, kExactBatch);
+  if (large) batch = std::min<int>(batch, std::max<int>(kExQB, static_cast<int>(kExactKeysBytes / per_query) / kExQB * kExQB));
+  int rc = ensure(&ix->chunk_keys, &ix->chunk_keys_elems, static_cast<size_t>(batch) * (n_chunks + 1) * ep.k);
+  if (rc) return rc;
+  ep.chunk_keys = ix->chunk_keys;
+  const int buf = large ? kExBufLarge : kExBufSmall;
+  const size_t smem = static_cast<size_t>(kExQB) * buf * 8 + static_cast<size_t>(kExQB) * d * 4;
+  auto chunk_kernel = large ? exact_chunk_kernel<kExBufLarge, true> : exact_chunk_kernel<kExBufSmall, true>;
+  ANCE_CUDA(cudaFuncSetAttribute(chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 large ? static_cast<int>(smem) : 100 * 1024));
+  float* stage = nullptr;
+  cudaError_t e = cudaMalloc(&stage, static_cast<size_t>(slab) * d * 4);
+  if (e != cudaSuccess) {
+    ance::set_error("ance_index_search_exact: cudaMalloc(%lld bytes) of the staging buffer failed: %s",
+                    (long long)(slab * d * 4), cudaGetErrorString(e));
+    return ANCE_ERR_NOMEM;
+  }
+  for (int b0 = 0; b0 < nq && e == cudaSuccess; b0 += batch) {
+    const int nb = std::min(batch, nq - b0);
+    ep.qlist = qlist ? qlist + b0 : nullptr;
+    ep.q_base = b0;
+    ep.nq = nb;
+    const int gy = std::max(1, std::min((nb + kExQB - 1) / kExQB, 128));
+    ance::ProfScope ps(ance::kClsExact, st);
+    e = cudaMemsetAsync(ep.chunk_keys, 0, static_cast<size_t>(nb) * (n_chunks + 1) * ep.k * 8, st);   // empty best-k slots
+    for (int64_t r0 = 0; r0 < n && e == cudaSuccess; r0 += slab) {
+      const int64_t m = std::min(slab, n - r0);
+      e = cudaMemcpyAsync(stage, ix->P32_host + r0 * d, static_cast<size_t>(m) * d * 4, cudaMemcpyHostToDevice, st);
+      if (e != cudaSuccess) break;
+      ep.P = stage;
+      ep.n_rows = m;
+      chunk_kernel<<<dim3(n_chunks, gy), 256, smem, st>>>(ep, r0);
+      ExactParams mp = ep;
+      mp.n_chunks = n_chunks + 1;   // the chunk keys and the running best-k slot
+      if (r0 + m < n)
+        exact_merge_kernel<true><<<std::max(1, std::min(nb, 4 * sms)), 256, 0, st>>>(mp, nullptr, nullptr, k, row_offset);
+      else
+        exact_merge_kernel<false><<<std::max(1, std::min(nb, 4 * sms)), 256, 0, st>>>(mp, D, I, k, row_offset);
+      ance::count_launch(2);
+      e = cudaGetLastError();
+    }
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);   // the staging buffer is in use until here
+  cudaFree(stage);
+  if (e != cudaSuccess) {
+    ance::set_error("ance_index_search_exact (host rows): %s", cudaGetErrorString(e));
+    return ANCE_ERR_CUDA;
+  }
+  return ANCE_OK;
+}
+
 int run_exact(ance_index* ix, const float* Q, const int* qlist, int nq, int k, float* D, int64_t* I,
               int64_t row_offset, cudaStream_t st) {
+  if (ix->host_rows) return run_exact_host(ix, Q, qlist, nq, k, D, I, row_offset, st);
   ExactParams ep;
   ep.Q = Q;
   ep.P = ix->P32;
@@ -955,10 +1226,9 @@ int run_exact(ance_index* ix, const float* Q, const int* qlist, int nq, int k, f
   const int buf = large ? kExBufLarge : kExBufSmall;
   const size_t smem = static_cast<size_t>(kExQB) * buf * 8 + static_cast<size_t>(kExQB) * ix->dim * 4;
   // per device and cheap: set on every call rather than behind a process-wide flag
-  if (large)
-    ANCE_CUDA(cudaFuncSetAttribute(exact_chunk_kernel<kExBufLarge>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  else
-    ANCE_CUDA(cudaFuncSetAttribute(exact_chunk_kernel<kExBufSmall>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+  auto chunk_kernel = large ? exact_chunk_kernel<kExBufLarge, false> : exact_chunk_kernel<kExBufSmall, false>;
+  ANCE_CUDA(cudaFuncSetAttribute(chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 large ? static_cast<int>(smem) : 100 * 1024));
   for (int b0 = 0; b0 < nq; b0 += batch) {
     const int nb = std::min(batch, nq - b0);
     ep.qlist = qlist ? qlist + b0 : nullptr;
@@ -966,10 +1236,9 @@ int run_exact(ance_index* ix, const float* Q, const int* qlist, int nq, int k, f
     ep.nq = nb;
     const int gy = std::max(1, std::min((nb + kExQB - 1) / kExQB, 128));
     ance::ProfScope ps(ance::kClsExact, st);
-    if (large) exact_chunk_kernel<kExBufLarge><<<dim3(n_chunks, gy), 256, smem, st>>>(ep);
-    else exact_chunk_kernel<kExBufSmall><<<dim3(n_chunks, gy), 256, smem, st>>>(ep);
+    chunk_kernel<<<dim3(n_chunks, gy), 256, smem, st>>>(ep, 0);
     ANCE_CUDA(cudaGetLastError());
-    exact_merge_kernel<<<std::max(1, std::min(nb, 4 * sms)), 256, 0, st>>>(ep, D, I, k, row_offset);
+    exact_merge_kernel<false><<<std::max(1, std::min(nb, 4 * sms)), 256, 0, st>>>(ep, D, I, k, row_offset);
     ANCE_CUDA(cudaGetLastError());
     ance::count_launch(2);
   }
@@ -1062,32 +1331,65 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
   rp.counters = ix->counters;
   rp.max_eps = reinterpret_cast<unsigned int*>(ix->counters + 2);
   rp.sort_n = next_pow2(ns * out_cap);
-  const size_t rs_smem = static_cast<size_t>(rp.sort_n) * 8 + static_cast<size_t>(ix->dim) * 4 + (ns + 1) * 4 + 16;
+  rp.P16 = ix->P16;
+  rp.ndelta = ix->ndelta;
+  rp.bf16 = bf;
+  size_t rs_smem = static_cast<size_t>(rp.sort_n) * 8 + static_cast<size_t>(ix->dim) * 4 + (ns + 1) * 4 + 16;
+  // host index: + per-candidate upper bounds (fp64), rows and survivors after the 16-byte aligned base layout
+  // (8192 candidates: 64 KB keys + 128 KB = 195 KB at d = 768)
+  if (ix->host_rows) rs_smem = ((rs_smem - 16 + 15) & ~size_t(15)) + static_cast<size_t>(rp.sort_n) * 16;
+  auto kern = ix->host_rows ? rescore_kernel<true> : rescore_kernel<false>;
   if (rs_smem > 48 * 1024)   // per device and cheap: no process-wide cache
-    ANCE_CUDA(cudaFuncSetAttribute(rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rs_smem)));
+    ANCE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rs_smem)));
   ance::prof_begin(ance::kClsRescore, st);
-  rescore_kernel<<<static_cast<unsigned>(nq), 256, rs_smem, st>>>(rp);
+  kern<<<static_cast<unsigned>(nq), 256, rs_smem, st>>>(rp);
   ance::prof_end(ance::kClsRescore, st);
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);
   return ANCE_OK;
 }
 
-int create_common(int dim, int64_t capacity_rows, int operand_fmt, float* external_rows, ance_index_t* out) {
+// host_rows: the fp32 rows live in pinned host memory (external_rows = caller-owned page-locked buffer, or null: allocated
+// here); otherwise external_rows is caller-owned device storage, or null: allocated here.
+int create_common(int dim, int64_t capacity_rows, int operand_fmt, float* external_rows, bool host_rows, ance_index_t* out) {
   ANCE_REQUIRE(out != nullptr, "ance_index_create: out is null");
   ANCE_REQUIRE(dim > 0 && dim % 8 == 0 && dim <= 4096, "ance_index_create: dim must be a multiple of 8 in (0, 4096], got %d", dim);
   ANCE_REQUIRE(capacity_rows > 0 && capacity_rows < (1ll << 31), "ance_index_create: capacity_rows out of range");
   ANCE_REQUIRE(operand_fmt == ANCE_FMT_BF16 || operand_fmt == ANCE_FMT_FP16, "ance_index_create: bad operand_fmt");
   int rc = check_device();
   if (rc) return rc;
+  float* host_dev = nullptr;   // device address of caller-owned host rows
+  if (host_rows && external_rows) {
+    cudaPointerAttributes a{};
+    const cudaError_t e = cudaPointerGetAttributes(&a, external_rows);
+    if (e != cudaSuccess) cudaGetLastError();   // not a sticky error: clear it
+    ANCE_REQUIRE(e == cudaSuccess && a.type == cudaMemoryTypeHost && a.devicePointer != nullptr &&
+                 (reinterpret_cast<uintptr_t>(external_rows) & 15) == 0,
+                 "ance_index_create_host: rows_host must be 16-byte aligned page-locked host memory mapped into the device");
+    host_dev = static_cast<float*>(a.devicePointer);
+  }
   ance_index* ix = new ance_index();
   ix->dim = dim;
   ix->cap = capacity_rows;
   ix->fmt = operand_fmt;
+  ix->host_rows = host_rows;
   cudaGetDevice(&ix->device);
   const size_t elems = static_cast<size_t>(capacity_rows) * dim;
   cudaError_t e1 = cudaSuccess;
-  if (external_rows) {
+  if (host_rows) {
+    ix->owns_p32 = false;
+    if (external_rows) {
+      ix->P32_host = external_rows;
+      ix->P32 = host_dev;
+    } else {
+      e1 = cudaHostAlloc(reinterpret_cast<void**>(&ix->P32_host), elems * 4, cudaHostAllocMapped | cudaHostAllocPortable);
+      if (e1 == cudaSuccess) {
+        ix->owns_host = true;
+        e1 = cudaHostGetDevicePointer(reinterpret_cast<void**>(&ix->P32), ix->P32_host, 0);
+      }
+    }
+    if (e1 == cudaSuccess) e1 = cudaMalloc(&ix->ndelta, static_cast<size_t>(capacity_rows) * sizeof(float));
+  } else if (external_rows) {
     ix->P32 = external_rows;
     ix->owns_p32 = false;
   } else {
@@ -1100,13 +1402,71 @@ int create_common(int dim, int64_t capacity_rows, int operand_fmt, float* extern
   cudaError_t e6 = cudaMalloc(&ix->mu, static_cast<size_t>(dim) * sizeof(float));
   cudaError_t e7 = cudaMalloc(&ix->colsum, static_cast<size_t>(dim) * sizeof(double));
   if (e1 || e2 || e3 || e4 || e5 || e6 || e7) {
-    ance::set_error("ance_index_create: cudaMalloc failed for %lld x %d rows", (long long)capacity_rows, dim);
+    ance::set_error("ance_index_create%s: %s failed for %lld x %d rows", host_rows ? "_host" : "",
+                    host_rows ? "cudaHostAlloc / cudaMalloc" : "cudaMalloc", (long long)capacity_rows, dim);
     ance_index_destroy(ix);
     return ANCE_ERR_NOMEM;
   }
   cudaMemset(ix->pstats, 0, 2 * sizeof(unsigned int));
   cudaMemset(ix->counters, 0, kNumCounters * sizeof(int));
   *out = ix;
+  return ANCE_OK;
+}
+
+// prepare_operands of a host index: the fp32 rows are streamed H2D in chunks through a staging buffer of at most 512 MB
+// (one pass for the column sums when centring, one for the rounding), and the same kernels as the device index's run on
+// each chunk.  The rounding also stores every row's ||delta_j|| (ndelta), which the rescoring pre-filter needs.  The
+// staging buffer is freed at the end: the index keeps 2 bytes per row element + 4 bytes per row on the device.
+int prepare_operands_host(ance_index* ix, cudaStream_t st) {
+  const int64_t n = ix->n;
+  if (n == 0) return ANCE_OK;
+  const int d = ix->dim;
+  const int64_t chunk = std::min<int64_t>(n, std::max<int64_t>(1, static_cast<int64_t>(kHostStageBytes / (static_cast<size_t>(d) * 4))));
+  float* stage = nullptr;
+  cudaError_t e = cudaMalloc(&stage, static_cast<size_t>(chunk) * d * 4);
+  if (e != cudaSuccess) {
+    ance::set_error("ance_index_prepare: cudaMalloc(%lld bytes) of the staging buffer failed: %s",
+                    (long long)(chunk * d * 4), cudaGetErrorString(e));
+    return ANCE_ERR_NOMEM;
+  }
+  auto stream_pass = [&](bool quantize) -> cudaError_t {
+    for (int64_t r0 = 0; r0 < n; r0 += chunk) {
+      const int64_t m = std::min(chunk, n - r0);
+      cudaError_t err = cudaMemcpyAsync(stage, ix->P32_host + r0 * d, static_cast<size_t>(m) * d * 4, cudaMemcpyHostToDevice, st);
+      if (err != cudaSuccess) return err;
+      if (!quantize) {
+        const int slab = static_cast<int>(std::min<int64_t>(4096, std::max<int64_t>(32, m / (8 * gemm::sm_count()))));
+        column_sum_kernel<<<static_cast<unsigned>((m + slab - 1) / slab), 256, 0, st>>>(stage, m, d, slab, ix->colsum);
+      } else {
+        const float* mu = ix->centred ? ix->mu : nullptr;
+        const unsigned blocks = static_cast<unsigned>((m + 7) / 8);
+        uint16_t* o16 = ix->P16 + r0 * d;
+        if (ix->fmt == ANCE_FMT_BF16)
+          quantize_rows_kernel<true><<<blocks, 256, 0, st>>>(stage, o16, m, d, mu, nullptr, ix->ndelta + r0, ix->pstats, ix->counters + kCntRowErr);
+        else
+          quantize_rows_kernel<false><<<blocks, 256, 0, st>>>(stage, o16, m, d, mu, nullptr, ix->ndelta + r0, ix->pstats, ix->counters + kCntRowErr);
+      }
+      ance::count_launch(1);
+      if ((err = cudaGetLastError()) != cudaSuccess) return err;
+    }
+    return cudaSuccess;
+  };
+  if (ix->centred) {
+    e = cudaMemsetAsync(ix->colsum, 0, static_cast<size_t>(d) * sizeof(double), st);
+    if (e == cudaSuccess) e = stream_pass(false);
+    if (e == cudaSuccess) {
+      finalize_mean_kernel<<<(d + 255) / 256, 256, 0, st>>>(ix->colsum, n, d, ix->mu);
+      ance::count_launch(1);
+      e = cudaGetLastError();
+    }
+  }
+  if (e == cudaSuccess) e = stream_pass(true);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);   // the staging buffer is in use until here
+  cudaFree(stage);
+  if (e != cudaSuccess) {
+    ance::set_error("ance_index_prepare (host rows): %s", cudaGetErrorString(e));
+    return ANCE_ERR_CUDA;
+  }
   return ANCE_OK;
 }
 
@@ -1120,6 +1480,12 @@ int prepare_operands(ance_index* ix, cudaStream_t st) {
   ANCE_CUDA(cudaMemsetAsync(ix->counters + kCntRowErr, 0, sizeof(int), st));
   ance::ProfScope ps(ance::kClsQuant, st);
   ix->centred = ix->center && n >= 256;
+  if (ix->host_rows) {
+    int rc = prepare_operands_host(ix, st);
+    if (rc) return rc;
+    ix->dirty = false;
+    return ANCE_OK;
+  }
   if (ix->centred) {
     ANCE_CUDA(cudaMemsetAsync(ix->colsum, 0, static_cast<size_t>(ix->dim) * sizeof(double), st));
     // rows per block: enough blocks to fill the machine for a small index, few enough atomics (n / slab per column) for a big one
@@ -1214,6 +1580,7 @@ int search_tiers(ance_index* ix, const float* q_dev, int64_t nq, int k, int kpri
     rc = run_exact(ix, q_dev, ix->flagged, n_exact, k, D_dev, I_dev, row_offset, st);
     if (rc) return rc;
   }
+  ix->last_fetched += h[kCntFetched];   // tiers 1 and 2 (the counters are cleared once per block, above)
   acc->n_splits = std::max(acc->n_splits, ns);
   acc->n_tier2 += h[0];
   acc->n_uncertified += n_exact;
@@ -1227,23 +1594,28 @@ int search_tiers(ance_index* ix, const float* q_dev, int64_t nq, int k, int kpri
 }  // namespace
 
 extern "C" int ance_index_create(int dim, int64_t capacity_rows, int operand_fmt, ance_index_t* out) {
-  return create_common(dim, capacity_rows, operand_fmt, nullptr, out);
+  return create_common(dim, capacity_rows, operand_fmt, nullptr, false, out);
+}
+
+extern "C" int ance_index_create_host(int dim, int64_t capacity_rows, int operand_fmt, float* rows_host, ance_index_t* out) {
+  return create_common(dim, capacity_rows, operand_fmt, rows_host, true, out);
 }
 
 extern "C" int ance_index_create_over(int dim, int64_t capacity_rows, int operand_fmt, float* rows_dev,
                                       ance_index_t* out) {
   ANCE_REQUIRE(rows_dev != nullptr, "ance_index_create_over: rows_dev is null");
   ANCE_REQUIRE((reinterpret_cast<uintptr_t>(rows_dev) & 15) == 0, "ance_index_create_over: rows_dev must be 16-byte aligned");
-  return create_common(dim, capacity_rows, operand_fmt, rows_dev, out);
+  return create_common(dim, capacity_rows, operand_fmt, rows_dev, false, out);
 }
 
 extern "C" int ance_index_destroy(ance_index_t ix) {
   if (!ix) return ANCE_OK;
   void* ptrs[] = {ix->owns_p32 ? ix->P32 : nullptr, ix->P16, ix->pstats, ix->Q16, ix->qn_hat, ix->qn_delta, ix->scratch_sc,
                   ix->scratch_id, ix->cand_id, ix->cand_cnt, ix->cand_thr, ix->flagged, ix->flagged_thr, ix->counters,
-                  ix->chunk_keys, ix->flagged2, ix->Q16b, ix->pace, ix->mu, ix->colsum};
+                  ix->chunk_keys, ix->flagged2, ix->Q16b, ix->pace, ix->mu, ix->colsum, ix->ndelta};
   for (void* p : ptrs)
     if (p) cudaFree(p);
+  if (ix->owns_host) cudaFreeHost(ix->P32_host);
   delete ix;
   return ANCE_OK;
 }
@@ -1270,7 +1642,13 @@ extern "C" int ance_index_add(ance_index_t ix, const float* rows_dev, int64_t n,
   if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* dst = ix->P32 + static_cast<size_t>(ix->n) * ix->dim;
-  if (dst != rows_dev)   // rows produced in place (the encoder wrote straight into the index storage): no copy
+  if (ix->host_rows) {
+    // device rows: stream-ordered D2H into the pinned storage; any other host pointer: a plain (synchronous) copy; the
+    // storage slice itself (host or device address): no copy
+    float* dst_host = ix->P32_host + static_cast<size_t>(ix->n) * ix->dim;
+    if (dst_host != rows_dev && dst != rows_dev)
+      ANCE_CUDA(cudaMemcpyAsync(dst_host, rows_dev, static_cast<size_t>(n) * ix->dim * 4, cudaMemcpyDefault, st));
+  } else if (dst != rows_dev)   // rows produced in place (the encoder wrote straight into the index storage): no copy
     ANCE_CUDA(cudaMemcpyAsync(dst, rows_dev, static_cast<size_t>(n) * ix->dim * 4, cudaMemcpyDeviceToDevice, st));
   ix->n += n;
   ix->dirty = true;      // the 16-bit operands are (re)built from all rows by the next ance_index_prepare / search
@@ -1340,6 +1718,7 @@ extern "C" int ance_index_search(ance_index_t ix, const float* q_dev, int64_t nq
   int rc = check_handle_device(ix, "ance_index_search");
   if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ix->last_fetched = 0;
   // choose k' (candidates kept per split).  The certificate needs every row within eps of the k-th score among the
   // candidates; eps is ~0.5 (fp16 operands) / ~3 (bf16) for rows of norm 27.7, i.e. ~0.1 k / ~0.6 k extra rows on the
   // distributions of tools/exp_certify.py.  A query that k' does not cover costs one tier-2 pass, not a wrong answer.
@@ -1389,3 +1768,22 @@ extern "C" int ance_index_last_stats(ance_index_t ix, ance_search_stats* out) {
   *out = ix->stats;
   return ANCE_OK;
 }
+
+extern "C" int ance_index_memory(ance_index_t ix, int64_t* device_bytes, int64_t* host_bytes) {
+  ANCE_REQUIRE(ix != nullptr && device_bytes != nullptr && host_bytes != nullptr, "ance_index_memory: null argument");
+  const int64_t cap = ix->cap, d = ix->dim;
+  int64_t dev = (ix->owns_p32 ? cap * d * 4 : 0) + cap * d * 2 + (ix->ndelta ? cap * 4 : 0);
+  dev += 2 * 4 + kMaxPace * 4 + kNumCounters * 4 + d * 4 + d * 8;                       // pstats, pace, counters, mu, colsum
+  dev += ix->q_cap * d * 2 + 2 * ix->q_cap * 4;                                          // query operands and norms
+  dev += 2 * static_cast<int64_t>(ix->scratch_elems) * 4;                                // coarse reservoirs
+  dev += static_cast<int64_t>(ix->cand_ids) * 4 + 2 * static_cast<int64_t>(ix->cand_slots) * 4;   // candidate lists
+  dev += 2 * ix->flagged_cap * 4 + static_cast<int64_t>(ix->flagged2_cap) * 4 + static_cast<int64_t>(ix->q16b_elems) * 2;
+  dev += static_cast<int64_t>(ix->chunk_keys_elems) * 8;                                 // brute-force keys
+  *device_bytes = dev;
+  *host_bytes = ix->owns_host ? cap * d * 4 : 0;
+  return ANCE_OK;
+}
+
+extern "C" int64_t ance_index_last_fetched(ance_index_t ix) { return ix ? ix->last_fetched : -1; }
+
+extern "C" float* ance_index_host_rows(ance_index_t ix) { return (ix && ix->host_rows) ? ix->P32_host : nullptr; }

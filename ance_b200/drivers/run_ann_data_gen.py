@@ -140,6 +140,38 @@ def rows_from_batches(emb: torch.Tensor, idx: np.ndarray, batch: int) -> Tuple[t
     return torch.cat(rows, dim=0), np.concatenate(ids)
 
 
+def device_memory_available(device) -> int:
+    """Bytes a new allocation can get on `device`: the driver's free memory plus what torch's caching allocator holds
+    reserved but unused (from the second refresh of the poll loop on, the previous refresh's rows sit there)."""
+    free, _ = torch.cuda.mem_get_info(device)
+    return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
+# device -> (operand, host index): the host index of the last refresh, reused by the next one when its capacity matches.
+# Every refresh of the poll loop builds a new backend, so this lives at module level; pinning tens of GB is slow
+# (tools/bench_host_rows.py: 64.6 GB in 31 s).  The library allocates exactly capacity x dim fp32.
+_HOST_INDEX: Dict[str, tuple] = {}
+
+
+def _host_index(dim: int, capacity: int, device, operand: str):
+    from ..search import IndexFlatIP
+    from .. import _lib
+    key = str(torch.device(device))
+    cached = _HOST_INDEX.pop(key, None)
+    if cached is not None and cached[0] == operand and cached[1].d == dim and cached[1]._capacity == capacity:
+        index = cached[1]
+        index.reset()
+        fmt = _lib.ANCE_FMT_BF16 if operand == "bf16" else _lib.ANCE_FMT_FP16
+        if index.operand != fmt:   # an "auto" index that switched to bf16 starts the next refresh at fp16 again
+            index.set_param("operand_fmt", fmt)
+            index.operand = fmt
+    else:
+        del cached   # release the old pinned rows before pinning new ones
+        index = IndexFlatIP(dim, capacity=capacity, device=device, operand=operand, rows="host")
+    _HOST_INDEX[key] = (operand, index)
+    return index
+
+
 class B200Backend:
     """Encode + search on this rank's GPU through libance_b200."""
 
@@ -180,19 +212,32 @@ class B200Backend:
         reader = StridedBatchReader(cache, per, rank=rank, world_size=W)
         n_rows = reader.n_local * C
         dim = 768
-        rows = torch.empty((max(n_rows, 1), dim), dtype=torch.float32, device=self.device)[:n_rows]
+        host = build_index and self.index_rows(n_rows, dim) == "host"
         index = None
-        if build_index:
-            from ..search import IndexFlatIP
-            index = IndexFlatIP(dim, device=self.device, operand=args.search_operand,
-                                storage=rows if n_rows else None, capacity=0 if n_rows else 1)
+        if host:
+            # host index: the fp32 rows live in the library's pinned host memory; every super-batch is encoded into a
+            # device staging slice and added, i.e. copied D2H into its place
+            index = _host_index(dim, max(n_rows, 1), self.device, args.search_operand)
+            rows = index.rows_tensor()[:n_rows]
+            stage = None
+        else:
+            rows = torch.empty((max(n_rows, 1), dim), dtype=torch.float32, device=self.device)[:n_rows]
+            if build_index:
+                from ..search import IndexFlatIP
+                index = IndexFlatIP(dim, device=self.device, operand=args.search_operand,
+                                    storage=rows if n_rows else None, capacity=0 if n_rows else 1)
         ids_out: List[np.ndarray] = []
         pos = 0
         with torch.no_grad():
             for ids, lens, idx in reader:
                 ids_d = ids.to(self.device, non_blocking=True)
                 lens_d = lens.to(self.device, non_blocking=True)
-                out = rows[pos:pos + ids.shape[0] * C]
+                if host:
+                    if stage is None or stage.shape[0] < ids.shape[0] * C:
+                        stage = torch.empty((ids.shape[0] * C, dim), dtype=torch.float32, device=self.device)
+                    out = stage[:ids.shape[0] * C]
+                else:
+                    out = rows[pos:pos + ids.shape[0] * C]
                 if self.mask_mode == "nonzero" and packed:
                     fn = self.model.query_emb_packed if is_query else self.model.body_emb_packed
                     out.copy_(fn(ids_d, align=16, ids_host=ids))
@@ -218,13 +263,24 @@ class B200Backend:
                     self.model.encode_lens(ids_d, lens_d, out=out)
                     i = idx.numpy()
                 if index is not None:
-                    index.add(out)     # in place: the slice already IS index storage (no copy; operands are built by prepare())
+                    index.add(out)     # device index: in place, the slice already IS index storage (no copy; operands
+                                       # are built by prepare()); host index: D2H into the pinned storage
                 ids_out.append(i)
                 pos += out.shape[0]
+        if host:
+            torch.cuda.current_stream(self.device).synchronize()   # the D2H copies into `rows` have landed
         if hasattr(self.model, "check_inputs"):
             self.model.check_inputs()   # out-of-vocabulary ids: fail like the reference's embedding lookup does
         emb2id = np.concatenate(ids_out) if ids_out else np.empty((0,), dtype=np.int64)
         return (index, rows, emb2id) if build_index else (rows, emb2id)
+
+    def index_rows(self, n_rows: int, dim: int) -> str:
+        """--index_rows: "device" or "host" for an index of n_rows rows.  auto = device whenever its 6 bytes per row
+        element (fp32 rows + 16-bit operands) plus the search workspace fit in the device memory available now."""
+        mode = getattr(self.args, "index_rows", "auto")
+        if mode != "auto":
+            return mode
+        return "device" if 6 * n_rows * dim + INDEX_WORKSPACE_RESERVE <= device_memory_available(self.device) else "host"
 
     def make_local_search(self, passages) -> Callable:
         """passages: an IndexFlatIP built by encode(build_index=True), or a [n, 768] CUDA tensor (copied into a new one)."""
@@ -508,7 +564,7 @@ def generate_new_ann(args, output_num, checkpoint_path, training_query_positive_
     t = lap("encode_train_query_s", t)
     t_enc = time.time()
 
-    device = p_emb.device
+    device = args.device   # the backend's device (p_emb is host memory with --index_rows host)
     local_search = backend.make_local_search(index)
     passage_embedding2id = all_gather_ids(p_ids, device)
     dev_all, dev_query_embedding2id = all_gather_rows(dev_emb), all_gather_ids(dev_ids, device)
@@ -561,6 +617,12 @@ def generate_new_ann(args, output_num, checkpoint_path, training_query_positive_
 # CLI (flags of run_ann_data_gen.py:443-627, plus three GPU knobs at the end)
 # =============================================================================================
 MAX_TOPK = 2048   # largest k ance_index_search serves
+# device memory kept free for the search workspace when --index_rows auto decides (include/ance_b200.h: about 2.2 GB)
+INDEX_WORKSPACE_RESERVE = int(2.25 * 2 ** 30)
+INDEX_ROWS_CHOICES = ["auto", "device", "host"]
+INDEX_ROWS_HELP = ("where the index keeps its fp32 rows: device (HBM, 6 bytes per row element on the device) or host "
+                   "(pinned host memory, 2 bytes per element + 4 per row on the device; same results); auto = device "
+                   "whenever that fits in the device memory available when the passage encode starts (free + cached by torch)")
 
 
 def topk_arg(v: str) -> int:
@@ -603,6 +665,7 @@ def get_arguments(argv=None):
                    help="16-bit operand format of the coarse tensor-core pass (results are exact either way); auto = fp16, "
                         "falling back to bf16 when a row or a query leaves the fp16 range")
     p.add_argument("--encode_batch_tokens", default=75776, type=int, help="tokens per encoder launch sequence")
+    p.add_argument("--index_rows", default="auto", choices=INDEX_ROWS_CHOICES, help=INDEX_ROWS_HELP)
     p.add_argument("--reference_sampling", default=False, action="store_true",
                    help="draw the negative-sampling order from Python's `random` exactly as the reference does")
     p.add_argument("--seed", default=None, type=int, help="seed for the sampling order (reference: unseeded)")

@@ -139,7 +139,7 @@ def generate_new_ann(args, output_num, checkpoint_path, preloaded_data, latest_s
     dev_emb, dev_ids = backend.encode(os.path.join(d, "test-query"), True)
     tv_emb, tv_ids = backend.encode(os.path.join(d, "trivia-test-query"), True)
     index, p_emb, p_ids = backend.encode(os.path.join(d, "passages"), False, build_index=True)
-    device = p_emb.device
+    device = args.device   # the backend's device (p_emb is host memory with --index_rows host)
     local_search = backend.make_local_search(index)
     passage_embedding2id = all_gather_ids(p_ids, device)
     sets = {}
@@ -200,6 +200,7 @@ def get_arguments(argv=None):
     # GPU knobs
     p.add_argument("--search_operand", default="auto", choices=["auto", "fp16", "bf16"])
     p.add_argument("--encode_batch_tokens", default=75776, type=int)
+    p.add_argument("--index_rows", default="auto", choices=base.INDEX_ROWS_CHOICES, help=base.INDEX_ROWS_HELP)
     p.add_argument("--seed", default=None, type=int)
     p.add_argument("--poll_seconds", default=60, type=int)
     a = p.parse_args(argv)

@@ -40,15 +40,25 @@ def _as_f32_cuda(x, device) -> torch.Tensor:
 
 
 class IndexFlatIP:
-    """Exact maximum-inner-product search over fp32 rows resident in HBM."""
+    """Exact maximum-inner-product search over fp32 rows resident in HBM, or in pinned host memory (rows="host")."""
 
     def __init__(self, d: int, capacity: int = 0, device: Optional[torch.device] = None,
-                 operand: str = "auto", storage: Optional[torch.Tensor] = None):
+                 operand: str = "auto", storage: Optional[torch.Tensor] = None, rows: str = "device"):
         """operand: 16-bit format of the coarse tensor-core pass — "fp16" (certificate error bound ~8x tighter than bf16:
         fewer candidates to rescore), "bf16" (any fp32 range), or "auto" = fp16, switching the whole index to bf16 the
         first time a row or a query does not fit the fp16 range.  Results are exact either way.
         storage: a CUDA fp32 tensor [capacity, d] to use as the index's row storage (kept alive by the index).  Rows
-        written into `storage[i:i+n]` by their producer and then passed to add() are added without a copy."""
+        written into `storage[i:i+n]` by their producer and then passed to add() are added without a copy.  A PINNED CPU
+        fp32 tensor selects a host index over it.
+        rows: "device" (fp32 rows in HBM: 6 bytes per row element on the device) or "host" (fp32 rows in pinned host
+        memory, allocated by the library unless `storage` is given: 2 bytes per element + 4 per row on the device, for
+        corpora the device cannot hold in fp32; same exact results)."""
+        if rows not in ("device", "host"):
+            raise ValueError(f"rows must be 'device' or 'host', got {rows!r}")
+        if storage is not None and storage.device.type == "cpu":
+            if not storage.is_pinned():
+                raise ValueError("a CPU storage tensor must be pinned (torch.empty(..., pin_memory=True))")
+            rows = "host"
         if not torch.cuda.is_available():
             raise _lib.AnceError("ance_b200.IndexFlatIP needs a CUDA device (sm_90); there is no CPU fallback")
         self._lib = _lib.load()
@@ -56,15 +66,19 @@ class IndexFlatIP:
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.auto_operand = operand == "auto"
         self.operand = {"bf16": _lib.ANCE_FMT_BF16, "fp16": _lib.ANCE_FMT_FP16, "auto": _lib.ANCE_FMT_FP16}[operand]
+        self.host_rows = rows == "host"
         self._h = None
         self._capacity = 0
         self.ntotal = 0
         self.storage = None
         if storage is not None:
-            if (storage.device.type != "cuda" or storage.dtype != torch.float32 or storage.dim() != 2
+            want = "cpu" if self.host_rows else "cuda"
+            if (storage.device.type != want or storage.dtype != torch.float32 or storage.dim() != 2
                     or storage.shape[1] != self.d or not storage.is_contiguous()):
-                raise ValueError("storage must be a contiguous CUDA float32 tensor [capacity, d]")
-            self.device = storage.device
+                raise ValueError(f"storage must be a contiguous {'pinned CPU' if self.host_rows else 'CUDA'} "
+                                 "float32 tensor [capacity, d]")
+            if not self.host_rows:
+                self.device = storage.device
             self.storage = storage
             capacity = storage.shape[0]
         if capacity:
@@ -74,7 +88,10 @@ class IndexFlatIP:
     def _create(self, capacity: int):
         h = C.c_void_p()
         with torch.cuda.device(self.device):
-            if self.storage is not None:
+            if self.host_rows:
+                _lib.check(self._lib.ance_index_create_host(self.d, capacity, self.operand, _lib.ptr(self.storage),
+                                                            C.byref(h)))
+            elif self.storage is not None:
                 _lib.check(self._lib.ance_index_create_over(self.d, capacity, self.operand, self.storage.data_ptr(),
                                                             C.byref(h)))
             else:
@@ -114,6 +131,17 @@ class IndexFlatIP:
             raise _lib.AnceError(f"index capacity {self._capacity} exceeded ({self.ntotal} + {n}); "
                                  "pass capacity= at construction")
         with torch.cuda.device(self.device):
+            if self.host_rows:
+                # CUDA rows: D2H in stream order; host rows (numpy / CPU tensor): one synchronous host copy; the
+                # storage slice itself: no copy
+                if isinstance(x, np.ndarray):
+                    x = torch.from_numpy(np.ascontiguousarray(x))
+                if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or x.dim() != 2:
+                    raise TypeError("expected a float32 [n, d] numpy array or torch tensor")
+                x = x.contiguous()
+                _lib.check(self._lib.ance_index_add(self._h, x.data_ptr(), n, _lib.current_stream()))
+                self.ntotal += n
+                return
             step = 1 << 20 if not (isinstance(x, torch.Tensor) and x.device.type == "cuda") else n
             for s in range(0, n, step):
                 xs = _as_f32_cuda(x[s:s + step], self.device)
@@ -177,6 +205,31 @@ class IndexFlatIP:
         s = _lib.SearchStats()
         _lib.check(self._lib.ance_index_last_stats(self._h, C.byref(s)))
         return {n: getattr(s, n) for n, _ in s._fields_}
+
+    def memory(self) -> dict:
+        """{"device": bytes, "host": bytes} this index allocated itself (rows, 16-bit operands, workspace so far; its
+        own pinned rows).  Caller-owned storage is not counted."""
+        if self._h is None:
+            return {"device": 0, "host": 0}
+        dev, host = C.c_int64(), C.c_int64()
+        _lib.check(self._lib.ance_index_memory(self._h, C.byref(dev), C.byref(host)))
+        return {"device": dev.value, "host": host.value}
+
+    def rows_tensor(self) -> torch.Tensor:
+        """Host index: its fp32 rows [capacity, d] as a CPU tensor over the pinned storage (no copy; the tensor keeps the
+        index alive).  Rows [0, ntotal) are valid once the copies of add() have completed on the stream."""
+        if not self.host_rows or self._h is None:
+            raise _lib.AnceError("rows_tensor() needs a host index with a capacity")
+        if self.storage is not None:
+            return self.storage
+        n = self._capacity * self.d
+        buf = (C.c_float * n).from_address(self._lib.ance_index_host_rows(self._h))
+        buf._index = self   # the library's allocation lives as long as the handle
+        return torch.frombuffer(buf, dtype=torch.float32, count=n).view(self._capacity, self.d)
+
+    def last_fetched(self) -> int:
+        """Rows the last search's rescoring read from host memory (0 for a device index)."""
+        return int(self._lib.ance_index_last_fetched(self._h)) if self._h is not None else 0
 
 
 def merge_topk_host(Ds, Is, k: int, n_threads: int = 0, out=None):

@@ -66,10 +66,26 @@ int ance_index_create(int dim, int64_t capacity_rows, int operand_fmt, ance_inde
  * corpus instead of the reference's three (per-batch arrays -> concatenation -> faiss storage,
  * drivers/run_ann_data_gen.py:160-193,271). */
 int ance_index_create_over(int dim, int64_t capacity_rows, int operand_fmt, float* rows_dev, ance_index_t* out);
+/* HOST index: the fp32 rows live in page-locked host memory, the device keeps only the coarse pass's 16-bit operands and
+ * 4 bytes per row (2 bytes per row element + 4 per row instead of 6 per element: 21,015,324 x 768 rows take 32.3 GB of
+ * device memory instead of 97 GB).  rows_host == NULL: the library allocates capacity_rows x dim fp32 with cudaHostAlloc
+ * and frees it in ance_index_destroy.  Otherwise rows_host is caller-owned page-locked memory mapped into the device
+ * (e.g. a torch pinned tensor; 16-byte aligned, else ANCE_ERR_INVALID) that must outlive the index.
+ * Results are the same exact top-k as a device index's.  What changes:
+ *   - ance_index_prepare streams the rows H2D through a device staging buffer of at most 512 MB (two passes over
+ *     4 * n * dim bytes when centring);
+ *   - rescoring (tiers 1 and 2) first bounds every candidate's score from its 16-bit row and residual norm in HBM and
+ *     reads over PCIe only the fp32 rows of candidates that can still reach the top k (ance_index_last_fetched);
+ *   - the brute force (tier 3, ance_index_search_exact) copies the rows H2D slab by slab (at most 512 MB of staging)
+ *     once per batch of <= 1024 queries (fewer for k > 512, as on a device index): one PCIe pass over the corpus per
+ *     batch (21M x 768 rows: 64.6 GB), acceptable for a fallback. */
+int ance_index_create_host(int dim, int64_t capacity_rows, int operand_fmt, float* rows_host, ance_index_t* out);
 int ance_index_destroy(ance_index_t idx);
 int ance_index_reset(ance_index_t idx);                       /* ntotal = 0, storage kept */
 int64_t ance_index_ntotal(ance_index_t idx);
-/* IndexFlatIP.add: append n rows (fp32, row-major [n, dim], device memory). */
+/* IndexFlatIP.add: append n rows (fp32, row-major [n, dim], device memory).  On a host index rows_dev may also be host
+ * memory: device rows are copied D2H in stream order, other host rows by a plain (synchronous) copy, and the storage
+ * slice rows_host + ntotal * dim itself is added without a copy. */
 int ance_index_add(ance_index_t idx, const float* rows_dev, int64_t n, void* stream);
 /* Build the 16-bit operands of the coarse pass from ALL rows added so far: the rows are centred on their column mean
  * (<q, p> = <q, p - mu> + <q, mu>: the ranking does not change, the certificate's error bound shrinks to the centred rows'
@@ -81,7 +97,7 @@ int ance_index_prepare(ance_index_t idx, void* stream);
  * evaluation, large --topk_training): reservoirs of 8192 entries, k' in [1024, 4096], queries processed in blocks of at
  * most 16,384 so that the workspace does not grow with nq; at k = 1000 and k = 2048 alike it peaks at about 2.2 GB on a
  * 132-SM H100 (reservoirs 1.11 GB, candidate ids <= 0.54 GB, brute-force keys <= 0.54 GB, query copies 0.05 GB), on top
- * of the index's own 6 bytes per row element. */
+ * of the index's own 6 bytes per row element (host index: 2 bytes per row element + 4 per row). */
 int ance_index_search(ance_index_t idx, const float* q_dev, int64_t nq, int k, float* D_dev, int64_t* I_dev,
                       int64_t row_offset, void* stream);
 /* Same contract (0 < k <= 2048), computed entirely by the exact fp32->fp64 brute-force kernel (validation path). */
@@ -89,6 +105,15 @@ int ance_index_search_exact(ance_index_t idx, const float* q_dev, int64_t nq, in
                             int64_t* I_dev, int64_t row_offset, void* stream);
 /* Statistics of the last search (ance_index_search has already synchronised its stream). */
 int ance_index_last_stats(ance_index_t idx, ance_search_stats* out);
+/* Memory the handle holds: *device_bytes = its own device allocations (rows it allocated, 16-bit operands, per-row norms,
+ * search workspace grown so far), *host_bytes = its own pinned allocation (0 for caller-owned or device rows).  Unlike
+ * cudaMemGetInfo this does not count other processes sharing the device. */
+int ance_index_memory(ance_index_t idx, int64_t* device_bytes, int64_t* host_bytes);
+/* Rows the last ance_index_search's rescoring (tiers 1 and 2) read from host memory; 0 for a device index. */
+int64_t ance_index_last_fetched(ance_index_t idx);
+/* Host address of a host index's fp32 rows [capacity_rows, dim] (the library's allocation or rows_host); NULL for a device
+ * index.  Valid until ance_index_destroy. */
+float* ance_index_host_rows(ance_index_t idx);
 /* Tunables: "kprime" (multiple of 32 in [0, 4096]; 0 = auto: about 1.44 k for fp16 operands, 2 k + 32 for bf16, at least
  * 1024 when k > 512; a value below k, or above 992 when k <= 512, sends the search to the brute force), "n_splits"
  * (0 = auto), "cta_group" (1|2),
