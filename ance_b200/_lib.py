@@ -100,6 +100,12 @@ SIGNATURES = {
                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ance_dbg_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                 C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ance_dbg_linear": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                  C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ance_dbg_attention": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ance_dbg_layer_norm": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                      C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 

@@ -439,6 +439,20 @@ struct ance_encoder {
 
 namespace {
 
+// ANCE_ERR_CUDA unless the current device is an sm_90 GPU (there is no CPU fallback)
+int require_sm90(int* dev_out) {
+  int dev = 0, major = 0, minor = 0;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) {
+    ance::set_error("device %d has compute capability %d.%d; libance_b200 is built for sm_90a only (no CPU fallback)", dev, major, minor);
+    return ANCE_ERR_CUDA;
+  }
+  if (dev_out) *dev_out = dev;
+  return ANCE_OK;
+}
+
 template <class T>
 T* dev_alloc(ance_encoder* e, size_t n) {
   void* p = nullptr;
@@ -462,9 +476,15 @@ uint16_t* upload_16(ance_encoder* e, const float* h, size_t n) {
   return d;
 }
 
-// one GEMM of the forward: C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ R)
-// 128 x 128 tile per CTA (the wgmma warpgroup holds the whole tile in registers: 128 fp32 accumulators per thread),
-// 4 operand stages, 4 epilogue warps reading the shared accumulator tile while the next tile is computed.
+// GELU form of the FFN-up epilogue: 2 = logistic form (|err| <= 3.7e-6), 1 = erfc form (|err| <= 7.1e-7)
+int gelu_form() {
+  static const int form = getenv("ANCE_B200_GELU") ? atoi(getenv("ANCE_B200_GELU")) : 2;
+  return form;
+}
+
+// one GEMM of the forward: C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ R); act is the epilogue's code: 0 none, 1 / 2 GELU
+// (see gelu_form).  128 x 128 tile per CTA (the wgmma warpgroup holds the whole tile in registers: 128 fp32 accumulators
+// per thread), 4 operand stages, 4 epilogue warps reading the shared accumulator tile while the next tile is computed.
 template <uint32_t FMT>
 int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
            const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls = ance::kClsGemm,
@@ -495,9 +515,7 @@ int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K
   p.ldc = N;
   p.ldc32 = N;
   p.ldr = static_cast<int>(ldr);
-  // 2 = logistic form (|err| <= 3.7e-6), 1 = erfc form (|err| <= 7e-7)
-  static const int gelu_form = getenv("ANCE_B200_GELU") ? atoi(getenv("ANCE_B200_GELU")) : 2;
-  p.act = act ? gelu_form : 0;
+  p.act = act;
   {
     ance::ProfScope ps(cls, st);
     ANCE_CUDA((gemm::launch<Ep, BN, STAGES, CG, EW, FMT>(tmA, tmB, ws, p, 0, st)));
@@ -547,6 +565,56 @@ int set_attention_attrs() {
   return ANCE_OK;
 }
 
+// The attention of one layer: ctx [n_tokens, 64 heads] = softmax(Q K^T / 8 + kbias) V over qkv [n_tokens, 3 * 64 heads].
+// Dense (row_lo null): sequences of L tokens back to back.  Variable-length packing (row_lo / row_hi, and tile_kv when
+// L > 128, see PackPlan): n_tokens = 128 * tiles.  Built once per forward, launched once per layer.
+struct AttentionLaunch {
+  CUtensorMap tmQKV, tmCTX;
+  attn::Params ap;
+  int grid;
+  bool packed, single;   // the attention_kernel<kPacked, kSingle> instantiation
+};
+
+int make_attention(AttentionLaunch& a, const uint16_t* qkv, uint16_t* ctx, int n_tokens, int L, int heads,
+                   const float* kbias, const int32_t* row_lo, const int32_t* row_hi, const int2* tile_kv) {
+  const int H = heads * attn::kDh;
+  if (!tc05_host::make_tmap_2d_16b(&a.tmQKV, qkv, n_tokens, 3 * H, 3 * H, attn::kTile)) {
+    ance::set_error("encoder: cuTensorMapEncodeTiled failed for QKV");
+    return ANCE_ERR_CUDA;
+  }
+  if (!tc05_host::make_tmap_2d_16b(&a.tmCTX, ctx, n_tokens, H, H, attn::kTile)) {
+    ance::set_error("encoder: cuTensorMapEncodeTiled failed for the attention output");
+    return ANCE_ERR_CUDA;
+  }
+  const bool varlen = row_lo != nullptr;
+  const bool varlen_long = varlen && L > attn::kTile;   // sequences may span several tiles: multi-block attention items
+  attn::Params& ap = a.ap;
+  ap.n_tokens = n_tokens; ap.L = (varlen && !varlen_long) ? 64 : L; ap.heads = heads; ap.hidden = H;   // varlen: any L < 128 selects the packed kernel
+  ap.kbias = kbias;
+  ap.scale_log2 = kLog2e / 8.0f;
+  ap.row_lo = varlen ? row_lo : nullptr;
+  ap.row_hi = varlen ? row_hi : nullptr;
+  ap.tile_kv = varlen ? tile_kv : nullptr;
+  const int attn_work = ((n_tokens + 127) / 128) * heads;
+  a.grid = std::min(attn_work, gemm::sm_count());
+  a.packed = varlen || L < attn::kTile;
+  a.single = !varlen_long && L <= attn::kTile;
+  return ANCE_OK;
+}
+
+template <uint32_t FMT>
+int run_attention(const AttentionLaunch& a, cudaStream_t st) {
+  ance::prof_begin(ance::kClsAttn, st);
+  if (a.packed && !a.single) attn::attention_kernel<true, false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else if (a.packed) attn::attention_kernel<true, true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else if (a.single) attn::attention_kernel<false, true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else attn::attention_kernel<false, false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  ance::prof_end(ance::kClsAttn, st);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
 // n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
 // token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
 template <uint32_t FMT>
@@ -583,37 +651,13 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);
   if (e->dbg && M <= e->dbg_tokens) ANCE_CUDA(cudaMemcpyAsync(e->dbg, e->X, static_cast<size_t>(M) * H * 2, cudaMemcpyDeviceToDevice, st));
-  // attention tensor map over the QKV buffer
-  CUtensorMap tmQKV;
-  if (!tc05_host::make_tmap_2d_16b(&tmQKV, e->QKV, M, 3 * H, 3 * H, attn::kTile)) {
-    ance::set_error("encoder: cuTensorMapEncodeTiled failed for QKV");
-    return ANCE_ERR_CUDA;
-  }
-  CUtensorMap tmCTX;
-  if (!tc05_host::make_tmap_2d_16b(&tmCTX, e->CTX, M, H, H, attn::kTile)) {
-    ance::set_error("encoder: cuTensorMapEncodeTiled failed for the attention output");
-    return ANCE_ERR_CUDA;
-  }
-  attn::Params ap;
-  ap.n_tokens = M; ap.L = (varlen && !varlen_long) ? 64 : L; ap.heads = c.heads; ap.hidden = H;   // varlen: any L < 128 selects the packed kernel
-  ap.kbias = e->kbias;
-  ap.scale_log2 = kLog2e / 8.0f;
-  ap.row_lo = varlen ? e->row_lo : nullptr;
-  ap.row_hi = varlen ? e->row_hi : nullptr;
-  ap.tile_kv = varlen ? e->tile_kv : nullptr;
-  const int attn_work = ((M + 127) / 128) * c.heads;
-  const int attn_grid = std::min(attn_work, gemm::sm_count());
+  AttentionLaunch attn_launch;
+  if ((rc = make_attention(attn_launch, e->QKV, e->CTX, M, L, c.heads, e->kbias, varlen ? e->row_lo : nullptr,
+                           varlen ? e->row_hi : nullptr, varlen ? e->tile_kv : nullptr))) return rc;
   for (int l = 0; l < c.n_layer; ++l) {
     const LayerDev& d = e->layers[l];
     if ((rc = linear<FMT>(e->X, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, e->QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
-    ance::prof_begin(ance::kClsAttn, st);
-    if (varlen_long) attn::attention_kernel<true, false, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
-    else if (varlen || L < attn::kTile) attn::attention_kernel<true, true, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
-    else if (L == attn::kTile) attn::attention_kernel<false, true, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
-    else attn::attention_kernel<false, false, FMT><<<attn_grid, attn::kThreads, attn::Smem::kDynamic, st>>>(tmQKV, tmCTX, ap);
-    ance::prof_end(ance::kClsAttn, st);
-    ANCE_CUDA(cudaGetLastError());
-    ance::count_launch(1);
+    if ((rc = run_attention<FMT>(attn_launch, st))) return rc;
     // In the last layer only token 0 of every sequence is read downstream (models.py:49,193): run the
     // out-projection, FFN and both LayerNorms on those B rows only (strided TMA views, compact outputs).
     const bool cls_only = (e->prune_last_layer || varlen) && (l == c.n_layer - 1);
@@ -630,7 +674,7 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
     }
     if ((rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, e->T, nullptr, st, ance::kClsGemmOut, pitch))) return rc;
     if ((rc = layer_norm<FMT>(e->T, false, H, Mr, H, d.ln1g, d.ln1b, c.ln_eps, e->X1, nullptr, st))) return rc;
-    if ((rc = linear<FMT>(e->X1, H, Mr, d.w1, F, H, d.b1, nullptr, 1, e->FF, nullptr, st, ance::kClsGemmFfn1))) return rc;
+    if ((rc = linear<FMT>(e->X1, H, Mr, d.w1, F, H, d.b1, nullptr, gelu_form(), e->FF, nullptr, st, ance::kClsGemmFfn1))) return rc;
     if ((rc = linear<FMT>(e->FF, F, Mr, d.w2, H, F, d.b2, e->X1, 0, e->T, nullptr, st, ance::kClsGemmFfn2))) return rc;
     if ((rc = layer_norm<FMT>(e->T, false, H, Mr, H, d.ln2g, d.ln2b, c.ln_eps, e->X, nullptr, st))) return rc;
     if (e->dbg && M <= e->dbg_tokens)  // with cls_only the first B rows hold the CLS rows of the last layer
@@ -671,17 +715,7 @@ extern "C" int ance_encoder_create(const ance_encoder_config* cfg, const ance_en
   ANCE_REQUIRE(!cfg->has_head || (w->head_w && w->head_b && w->head_ln_g && w->head_ln_b), "ance_encoder_create: has_head without head weights");
   ANCE_REQUIRE(cfg->operand_fmt == ANCE_FMT_FP16 || cfg->operand_fmt == ANCE_FMT_BF16, "ance_encoder_create: operand_fmt must be ANCE_FMT_FP16 or ANCE_FMT_BF16, got %d", cfg->operand_fmt);
   int dev = 0;
-  {
-    int major = 0;
-    ANCE_CUDA(cudaGetDevice(&dev));
-    cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    int minor = 0;
-    cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-    if (major != 9 || minor != 0) {
-      ance::set_error("device %d has compute capability %d.%d; libance_b200 is built for sm_90a only (no CPU fallback)", dev, major, minor);
-      return ANCE_ERR_CUDA;
-    }
-  }
+  if (const int rc = require_sm90(&dev)) return rc;
   ance_encoder* e = new ance_encoder();
   e->cfg = *cfg;
   e->device = dev;
@@ -1037,4 +1071,89 @@ extern "C" int ance_encoder_debug_hidden(ance_encoder_t e, int layer, float* out
   else act16_to_f32_kernel<tc05::kFmtF16><<<blocks, 256, 0, st>>>(e->dbg + static_cast<size_t>(layer) * n, out_dev, n);
   ANCE_CUDA(cudaGetLastError());
   return ANCE_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// test hooks: the encoder's own GEMM, attention and LayerNorm launches on caller buffers
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+}  // namespace
+
+extern "C" int ance_dbg_linear(int fmt, const void* A_dev, int64_t lda, int M, const void* W_dev, int N, int K,
+                               const float* bias_dev, const void* R_dev, int64_t ldr, int act, void* C16_dev,
+                               float* C32_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_linear: unknown operand format %d", fmt);
+  ANCE_REQUIRE(A_dev && W_dev && (C16_dev || C32_dev), "ance_dbg_linear: null operand or no output");
+  ANCE_REQUIRE(M > 0 && N > 0 && K > 0 && K % 8 == 0 && N % 8 == 0, "ance_dbg_linear: need M, N, K > 0 and N, K multiples of 8 (M=%d N=%d K=%d)", M, N, K);
+  ANCE_REQUIRE(lda >= K && lda % 8 == 0, "ance_dbg_linear: lda = %lld must be >= K = %d and a multiple of 8", static_cast<long long>(lda), K);
+  ANCE_REQUIRE(!R_dev || (ldr >= N && ldr % 8 == 0 && ldr <= INT32_MAX), "ance_dbg_linear: ldr = %lld must be >= N = %d and a multiple of 8", static_cast<long long>(ldr), N);
+  ANCE_REQUIRE(act >= 0 && act <= 2, "ance_dbg_linear: act must be 0 (none), 1 (GELU, erfc form) or 2 (GELU, logistic form), got %d", act);
+  ANCE_REQUIRE(aligned16(A_dev) && aligned16(W_dev) && aligned16(bias_dev) && aligned16(R_dev) && aligned16(C16_dev) && aligned16(C32_dev),
+               "ance_dbg_linear: every buffer must be 16-byte aligned");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* A = reinterpret_cast<const uint16_t*>(A_dev);
+  const auto* W = reinterpret_cast<const uint16_t*>(W_dev);
+  const auto* R = reinterpret_cast<const uint16_t*>(R_dev);
+  auto* C = reinterpret_cast<uint16_t*>(C16_dev);
+  const size_t ldr_ = R ? static_cast<size_t>(ldr) : 0;
+  if (fmt == ANCE_FMT_BF16) return linear<tc05::kFmtBF16>(A, static_cast<size_t>(lda), M, W, N, K, bias_dev, R, act, C, C32_dev, st, ance::kClsGemm, ldr_);
+  return linear<tc05::kFmtF16>(A, static_cast<size_t>(lda), M, W, N, K, bias_dev, R, act, C, C32_dev, st, ance::kClsGemm, ldr_);
+}
+
+extern "C" int ance_dbg_attention(int fmt, const void* qkv_dev, int n_tokens, int L, int heads, const float* kbias_dev,
+                                  const int32_t* row_lo_dev, const int32_t* row_hi_dev, const int32_t* tile_kv_dev,
+                                  void* ctx_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_attention: unknown operand format %d", fmt);
+  ANCE_REQUIRE(qkv_dev && ctx_dev && kbias_dev, "ance_dbg_attention: null buffer");
+  ANCE_REQUIRE(aligned16(qkv_dev) && aligned16(ctx_dev), "ance_dbg_attention: qkv and ctx must be 16-byte aligned");
+  ANCE_REQUIRE(heads >= 1 && heads <= 16, "ance_dbg_attention: heads = %d outside [1, 16]", heads);
+  ANCE_REQUIRE(n_tokens > 0 && L > 0 && L <= 512, "ance_dbg_attention: need n_tokens > 0 and 0 < L <= 512 (n_tokens = %d, L = %d)", n_tokens, L);
+  const bool varlen = row_lo_dev != nullptr;
+  if (varlen) {
+    ANCE_REQUIRE(row_hi_dev && n_tokens % attn::kTile == 0, "ance_dbg_attention: a row plan needs row_hi and n_tokens a multiple of 128");
+    ANCE_REQUIRE((L > attn::kTile) == (tile_kv_dev != nullptr), "ance_dbg_attention: tile_kv is required for L > 128 and only then");
+  } else {
+    ANCE_REQUIRE(!row_hi_dev && !tile_kv_dev, "ance_dbg_attention: row_hi / tile_kv without row_lo");
+    ANCE_REQUIRE((L % attn::kTile == 0) || (attn::kTile % L == 0 && L >= 8), "ance_dbg_attention: L = %d unsupported (need a multiple of 128 up to 512, or a divisor of 128)", L);
+    ANCE_REQUIRE(n_tokens % L == 0, "ance_dbg_attention: n_tokens = %d is not a multiple of L = %d", n_tokens, L);
+  }
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  AttentionLaunch a;
+  int rc = make_attention(a, reinterpret_cast<const uint16_t*>(qkv_dev), reinterpret_cast<uint16_t*>(ctx_dev), n_tokens, L,
+                          heads, kbias_dev, row_lo_dev, row_hi_dev, reinterpret_cast<const int2*>(tile_kv_dev));
+  if (rc) return rc;
+  if (fmt == ANCE_FMT_BF16) {
+    if ((rc = set_attention_attrs<tc05::kFmtBF16>())) return rc;
+    return run_attention<tc05::kFmtBF16>(a, st);
+  }
+  if ((rc = set_attention_attrs<tc05::kFmtF16>())) return rc;
+  return run_attention<tc05::kFmtF16>(a, st);
+}
+
+extern "C" int ance_dbg_layer_norm(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
+                                   const float* gamma_dev, const float* beta_dev, float eps, void* out16_dev,
+                                   float* out32_dev, int rows_per_warp, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_layer_norm: unknown operand format %d", fmt);
+  ANCE_REQUIRE(in_dev && gamma_dev && beta_dev && (out16_dev || out32_dev), "ance_dbg_layer_norm: null buffer or no output");
+  ANCE_REQUIRE(rows > 0 && H > 0 && H % 256 == 0 && H <= 1024, "ance_dbg_layer_norm: need rows > 0 and H in {256, 512, 768, 1024} (rows = %d, H = %d)", rows, H);
+  ANCE_REQUIRE(in_ld >= H && in_ld % 8 == 0, "ance_dbg_layer_norm: in_ld = %lld must be >= H and a multiple of 8", static_cast<long long>(in_ld));
+  ANCE_REQUIRE(rows_per_warp >= 1 && rows_per_warp <= 4, "ance_dbg_layer_norm: rows_per_warp must be 1, 2, 3 or 4, got %d", rows_per_warp);
+  ANCE_REQUIRE(aligned16(in_dev) && aligned16(gamma_dev) && aligned16(beta_dev) && aligned16(out16_dev) && aligned16(out32_dev),
+               "ance_dbg_layer_norm: every buffer must be 16-byte aligned");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int saved = g_ln_rows_per_warp;
+  g_ln_rows_per_warp = rows_per_warp;
+  const int rc = (fmt == ANCE_FMT_BF16)
+                     ? layer_norm<tc05::kFmtBF16>(in_dev, in_f32 != 0, static_cast<size_t>(in_ld), rows, H, gamma_dev, beta_dev, eps,
+                                                  reinterpret_cast<uint16_t*>(out16_dev), out32_dev, st)
+                     : layer_norm<tc05::kFmtF16>(in_dev, in_f32 != 0, static_cast<size_t>(in_ld), rows, H, gamma_dev, beta_dev, eps,
+                                                 reinterpret_cast<uint16_t*>(out16_dev), out32_dev, st);
+  g_ln_rows_per_warp = saved;
+  return rc;
 }

@@ -48,8 +48,8 @@ __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
 
 // HF "gelu" = x * 0.5 * (1 + erf(x / sqrt(2))) = relu(x) - 0.5 |x| erfc(|x| / sqrt(2)), with
 //   erfc(z) ~= (1 + a1 z + ... + a6 z^6)^-16        (Abramowitz & Stegun 7.1.28, |error| <= 3e-7)
-// and the 1/sqrt(2) folded into the coefficients.  Measured |error| of the GELU <= 7.1e-7 absolute (three
-// orders of magnitude below the bf16 rounding of the output).  The epilogue of the FFN-up GEMM is bound by
+// and the 1/sqrt(2) folded into the coefficients.  |error| of the GELU <= 7.1e-7 absolute (three orders of magnitude
+// below the bf16 rounding of the output; tests/test_encoder_refs_cpu.py checks the bound from these coefficients).  The epilogue of the FFN-up GEMM is bound by
 // the SFU (MUFU) rate, so this form uses ONE MUFU (rcp) per element and no exponential; everything else is
 // FFMA/FMUL: per PAIR of elements 28 fp32 ops + 2 LOP + 2 MUFU.RCP.
 __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {

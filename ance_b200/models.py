@@ -126,6 +126,10 @@ class _CudaEncoder:
         w.layers = lw
         if head is not None:
             lin, norm = head
+            if tuple(lin.weight.shape) != (H, H) or tuple(norm.weight.shape) != (H,):
+                # ance_encoder_create reads a hidden x hidden head: any other shape would be read out of bounds
+                raise _lib.AnceError(f"the CUDA encoder's head must be Linear({H}, {H}) + LayerNorm({H}), got "
+                                     f"weight {tuple(lin.weight.shape)}")
             w.head_w, w.head_b = fp(lin.weight), fp(lin.bias)
             w.head_ln_g, w.head_ln_b = fp(norm.weight), fp(norm.bias)
         self.hidden_size = H

@@ -171,7 +171,7 @@ typedef struct {
 typedef struct {
   const float *word_emb, *pos_emb, *type_emb, *emb_ln_g, *emb_ln_b;
   const ance_layer_weights* layers;                 /* [n_layer] */
-  const float *head_w, *head_b, *head_ln_g, *head_ln_b; /* embeddingHead, norm (has_head only) */
+  const float *head_w, *head_b, *head_ln_g, *head_ln_b; /* embeddingHead [hidden, hidden] + [hidden], norm [hidden] (has_head only) */
 } ance_encoder_weights;
 
 int ance_encoder_create(const ance_encoder_config* cfg, const ance_encoder_weights* w, int max_tokens,
@@ -236,8 +236,6 @@ int ance_profile_read(double* ms_by_class, int64_t* launches_by_class, int n, in
 /* ------------------------------------------------------------------------------------------------
  * Bring-up / test hooks (not part of the drop-in surface)
  * ------------------------------------------------------------------------------------------------ */
-/* D[M,N] = act(A[M,K] * B[N,K]^T + bias) + R ; A,B 16-bit device arrays in `fmt`; outputs optional.
- * variant: 0 = BN 256 CG 1, 1 = BN 128 CG 1, 2 = BN 256 CG 2, 3 = BN 128 CG 2, 4 = BN 64 CG 1 */
 /* Host-only: the tile plan ance_encoder_forward_varlen makes for the first chunk of lens_host[0..B) on a handle created with
  * `max_tokens`: row0_out[i] = packed row of sequence i's first token (i < *n_placed), lo/hi_out [*n_tiles * 128] = own-sequence
  * key range of every packed row (may be null). */
@@ -249,9 +247,34 @@ int ance_dbg_pack_varlen(const int32_t* lens_host, int B, int max_tokens, int al
  * items.  The three arrays may be null. */
 int ance_dbg_pack_packed(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
                          int32_t* lo_out, int32_t* hi_out, int32_t* tile_kv_out, int* n_placed, int* n_tiles);
+/* D[M,N] = act(A[M,K] * B[N,K]^T + bias) + R ; A,B 16-bit device arrays in `fmt`; R and the 16-bit output D are bf16
+ * whatever `fmt` is; outputs optional; act 0 none, 1 GELU (erfc form), 2 GELU (logistic form).
+ * variant (N tile BN, CTA cluster CG, operand stages): 0 = BN 128 CG 1 4 stages, 1 = BN 128 CG 1 3 stages,
+ * 2 = BN 128 CG 2 4 stages, 3 = BN 64 CG 2 6 stages, 4 = BN 64 CG 1 6 stages */
 int ance_dbg_gemm(const void* A_dev, const void* B_dev, int M, int N, int K, int fmt, int variant,
                   const float* bias_dev, const void* residual_bf16_dev, int act, void* C_bf16_dev,
                   float* C_f32_dev, void* stream);
+/* The encoder's own GEMM launch (the instantiation every linear layer of the forward runs):
+ * C[M,N] = act(A[M,K] W[N,K]^T + bias) + R with A rows at pitch lda, R rows at pitch ldr (ignored without R), C16 / C32
+ * at pitch N.  A, W, R and C16 are 16-bit in `fmt`, bias and C32 fp32; bias, R and either output may be null.  act: 0 none,
+ * 1 GELU (erfc form), 2 GELU (logistic form, the forward's default); the ANCE_B200_GELU environment variable is not read.
+ * Every buffer 16-byte aligned, N, K, lda, ldr multiples of 8. */
+int ance_dbg_linear(int fmt, const void* A_dev, int64_t lda, int M, const void* W_dev, int N, int K, const float* bias_dev,
+                    const void* R_dev, int64_t ldr, int act, void* C16_dev, float* C32_dev, void* stream);
+/* The encoder's own attention launch (same kernel selection and parameters as the forward): qkv [n_tokens, 3 * 64 heads]
+ * 16-bit (Q | K | V, head-major inside each), kbias [n_tokens] fp32 additive key bias in log2 units (0 or
+ * -10000 log2 e), ctx [n_tokens, 64 heads] 16-bit.  Dense (row_lo null): n_tokens / L sequences of L tokens.  Packed: the
+ * device row plan of ance_dbg_pack_packed (row_lo / row_hi [n_tokens], absolute rows; tile_kv [n_tokens / 128 * 2], only
+ * and always for L > 128), n_tokens a multiple of 128. */
+int ance_dbg_attention(int fmt, const void* qkv_dev, int n_tokens, int L, int heads, const float* kbias_dev,
+                       const int32_t* row_lo_dev, const int32_t* row_hi_dev, const int32_t* tile_kv_dev, void* ctx_dev,
+                       void* stream);
+/* The encoder's own LayerNorm launch: rows of `in` (16-bit in `fmt`, or fp32 when in_f32) at pitch in_ld -> out16 (16-bit)
+ * and / or out32 (fp32) at pitch H, H in {256, 512, 768, 1024}.  rows_per_warp (1..4) stands in for the process-wide
+ * "ln_rows_per_warp" tunable for this call only. */
+int ance_dbg_layer_norm(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H, const float* gamma_dev,
+                        const float* beta_dev, float eps, void* out16_dev, float* out32_dev, int rows_per_warp,
+                        void* stream);
 
 #ifdef __cplusplus
 }
