@@ -54,6 +54,17 @@ class EncoderWeights(C.Structure):
         ("layers", C.POINTER(LayerWeights))] + [(n, _FP) for n in ("head_w", "head_b", "head_ln_g", "head_ln_b")]
 
 
+class LayerGrads(C.Structure):
+    """ance_layer_grads: the layout of LayerWeights, device fp32 pointers."""
+    _fields_ = LayerWeights._fields_
+
+
+class EncoderGrads(C.Structure):
+    """ance_encoder_grads: the layout of EncoderWeights, device fp32 pointers."""
+    _fields_ = [(n, _FP) for n in ("word_emb", "pos_emb", "type_emb", "emb_ln_g", "emb_ln_b")] + [
+        ("layers", C.POINTER(LayerGrads))] + [(n, _FP) for n in ("head_w", "head_b", "head_ln_g", "head_ln_b")]
+
+
 # name -> (restype, argtypes); also the list the "-m 'not gpu'" symbol test checks against the header
 SIGNATURES = {
     "ance_version": (C.c_char_p, []),
@@ -92,6 +103,11 @@ SIGNATURES = {
     "ance_encoder_set_param": (C.c_int, [C.c_void_p, C.c_char_p, C.c_double]),
     "ance_encoder_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ance_encoder_debug_hidden": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_encoder_train_workspace": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ance_encoder_forward_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ance_encoder_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(EncoderGrads), C.c_void_p]),
+    "ance_encoder_update_weights": (C.c_int, [C.c_void_p, C.POINTER(EncoderWeights), C.c_void_p]),
     "ance_profile_enable": (C.c_int, [C.c_int]),
     "ance_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "ance_dbg_pack_varlen": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -106,6 +122,15 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ance_dbg_layer_norm": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "ance_dbg_attention_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                              C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_dbg_layer_norm_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                               C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
+    "ance_dbg_gelu_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "ance_dbg_embedding_backward": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p] * 8),
+    "ance_dbg_transpose_bf16": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                          C.c_void_p]),
 }
 
 

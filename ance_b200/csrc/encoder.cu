@@ -22,6 +22,7 @@
 
 #include "attention.cuh"
 #include "common.h"
+#include "encoder_bwd.cuh"
 #include "gemm_store.cuh"
 
 namespace {
@@ -435,6 +436,17 @@ struct ance_encoder {
   int prune_last_layer = 1;  // last layer: only the CLS rows go through out-proj / FFN (identical result)
   int varlen_align = 1;      // ance_encoder_forward_varlen / _packed: 1 = densest, 16 = exact packing, see pack_chunk
   std::vector<void*> allocs;
+  // training (ance_encoder_forward_train / _backward)
+  std::map<const void*, int2> train_shapes;   // workspace -> (B, L) of a forward_train whose backward has not run yet
+  struct LayerT { uint16_t *wqkv, *wo, *w1, *w2; };   // bf16 W^T: [H,3H] [H,H] [H,F] [F,H]
+  std::vector<LayerT> wt;                     // empty until the first backward
+  uint16_t* head_wt = nullptr;
+  bool wt_stale = true;                       // the W^T copies no longer match the weights
+  void* bwd_scratch = nullptr;                // backward scratch (ance_encoder_destroy frees it)
+  std::vector<bwd::RefreshPiece> refresh_table;   // ance_encoder_update_weights: the last table uploaded
+  bwd::RefreshPiece* refresh_dev = nullptr;       // its device copy (ance_encoder_destroy frees it)
+  size_t refresh_cap = 0;
+  size_t bwd_scratch_bytes = 0;
 };
 
 namespace {
@@ -615,11 +627,59 @@ int run_attention(const AttentionLaunch& a, cudaStream_t st) {
   return ANCE_OK;
 }
 
+// What the training forward keeps for the backward, in the caller's workspace (M = B * L tokens, byte offsets):
+//   ids [M] int32, kbias [M] fp32, then per layer the layer input X, QKV, CTX (M rows) and the LayerNorm inputs T1 / T2,
+//   the LayerNorm-1 output X1, the FFN-up pre-activation U and GELU output FF (M rows reserved, B used in the pruned last
+//   layer), then the last layer's CLS outputs [B, H] and the head LayerNorm's fp32 input [B, H].  Activations are 16-bit
+//   (operand_fmt).  LayerNorm statistics and softmax statistics are not stored: the backward recomputes them.
+struct TrainLayout {
+  size_t ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total;
+};
+
+TrainLayout train_layout(const ance_encoder_config& c, int B, int L) {
+  const size_t M = static_cast<size_t>(B) * L, H = c.hidden, F = c.ffn;
+  auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  TrainLayout t;
+  size_t o = 0;
+  t.ids = o; o += up(M * 4);
+  t.kbias = o; o += up(M * 4);
+  t.layers = o;
+  size_t p = 0;
+  t.x_in = p; p += up(M * H * 2);
+  t.qkv = p; p += up(M * 3 * H * 2);
+  t.ctx = p; p += up(M * H * 2);
+  t.t1 = p; p += up(M * H * 2);
+  t.x1 = p; p += up(M * H * 2);
+  t.u = p; p += up(M * F * 2);
+  t.ff = p; p += up(M * F * 2);
+  t.t2 = p; p += up(M * H * 2);
+  t.per_layer = p;
+  o += p * c.n_layer;
+  t.x_final = o; o += up(static_cast<size_t>(B) * H * 2);
+  t.head_in = o; o += up(static_cast<size_t>(B) * H * 4);
+  t.total = o;
+  return t;
+}
+
+struct TrainSave {
+  uint8_t* ws;
+  TrainLayout lo;
+  int n_layer;
+  uint16_t* at(int l, size_t off) const { return reinterpret_cast<uint16_t*>(ws + lo.layers + l * lo.per_layer + off); }
+  uint16_t* x(int l) const { return l == n_layer ? reinterpret_cast<uint16_t*>(ws + lo.x_final) : at(l, lo.x_in); }
+  int32_t* ids() const { return reinterpret_cast<int32_t*>(ws + lo.ids); }
+  float* kbias() const { return reinterpret_cast<float*>(ws + lo.kbias); }
+  float* head_in() const { return reinterpret_cast<float*>(ws + lo.head_in); }
+};
+
 // n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
 // token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
+// ts != null (dense, L <= 128): the training forward — the same launches on the same inputs, with every activation the
+// backward needs written to its own slot of the workspace instead of the reused buffers of the handle (plus the FFN-up
+// GEMM once more without GELU for the pre-activation), and the last layer always pruned to the CLS rows.
 template <uint32_t FMT>
 int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev, int B, int L,
-                 float* out_dev, cudaStream_t st, int n_tiles = 0) {
+                 float* out_dev, cudaStream_t st, int n_tiles = 0, const TrainSave* ts = nullptr) {
   const ance_encoder_config& c = e->cfg;
   const bool varlen = n_tiles > 0;
   const bool varlen_long = varlen && L > attn::kTile;   // sequences may span several tiles: multi-block attention items
@@ -631,13 +691,14 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   }
   // K1
   EmbedParams ep;
+  if (ts) ANCE_CUDA(cudaMemcpyAsync(ts->ids(), ids_dev, static_cast<size_t>(M) * 4, cudaMemcpyDeviceToDevice, st));
   ep.ids = ids_dev; ep.lens = lens_dev; ep.mask = mask_dev;
   ep.B = B; ep.L = L; ep.H = H;
   ep.roberta = (c.arch == ANCE_ARCH_ROBERTA);
   ep.pad_id = c.pad_id; ep.vocab = c.vocab; ep.max_pos = c.max_pos;
   ep.word = e->word; ep.pos = e->pos; ep.type = e->type;
   ep.gamma = e->eg; ep.beta = e->eb; ep.eps = c.ln_eps;
-  ep.X = e->X; ep.kbias = e->kbias; ep.err_flag = e->err_flag;
+  ep.X = ts ? ts->x(0) : e->X; ep.kbias = ts ? ts->kbias() : e->kbias; ep.err_flag = e->err_flag;
   ep.seq_row0 = varlen ? e->seq_row0 : nullptr;
   ep.long_pad = (varlen_long && e->varlen_align == 16) ? 32 : 0;
   ance::prof_begin(ance::kClsNorm, st);
@@ -656,13 +717,22 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
                            varlen ? e->row_hi : nullptr, varlen ? e->tile_kv : nullptr))) return rc;
   for (int l = 0; l < c.n_layer; ++l) {
     const LayerDev& d = e->layers[l];
-    if ((rc = linear<FMT>(e->X, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, e->QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
+    uint16_t* X_in = ts ? ts->x(l) : e->X;
+    uint16_t* QKV = ts ? ts->at(l, ts->lo.qkv) : e->QKV;
+    uint16_t* CTX = ts ? ts->at(l, ts->lo.ctx) : e->CTX;
+    uint16_t* T1 = ts ? ts->at(l, ts->lo.t1) : e->T;
+    uint16_t* X1 = ts ? ts->at(l, ts->lo.x1) : e->X1;
+    uint16_t* FF = ts ? ts->at(l, ts->lo.ff) : e->FF;
+    uint16_t* T2 = ts ? ts->at(l, ts->lo.t2) : e->T;
+    uint16_t* X_out = ts ? ts->x(l + 1) : e->X;
+    if (ts && (rc = make_attention(attn_launch, QKV, CTX, M, L, c.heads, ts->kbias(), nullptr, nullptr, nullptr))) return rc;
+    if ((rc = linear<FMT>(X_in, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
     if ((rc = run_attention<FMT>(attn_launch, st))) return rc;
     // In the last layer only token 0 of every sequence is read downstream (models.py:49,193): run the
     // out-projection, FFN and both LayerNorms on those B rows only (strided TMA views, compact outputs).
-    const bool cls_only = (e->prune_last_layer || varlen) && (l == c.n_layer - 1);
+    const bool cls_only = (e->prune_last_layer || varlen || ts) && (l == c.n_layer - 1);
     const int Mr = cls_only ? B : M;                                    // rows processed from here on
-    const uint16_t *ctx_a = e->CTX, *res_x = e->X;
+    const uint16_t *ctx_a = CTX, *res_x = X_in;
     size_t pitch = cls_only ? static_cast<size_t>(L) * H : H;           // row pitch of CTX / X views
     if (cls_only && varlen) {   // the CLS rows sit at seq_row0[b]: gather them into compact [B, H] operands
       ance::ProfScope ps(ance::kClsNorm, st);
@@ -672,23 +742,26 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
       ance::count_launch(2);
       ctx_a = e->cls_ctx; res_x = e->cls_x; pitch = H;
     }
-    if ((rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, e->T, nullptr, st, ance::kClsGemmOut, pitch))) return rc;
-    if ((rc = layer_norm<FMT>(e->T, false, H, Mr, H, d.ln1g, d.ln1b, c.ln_eps, e->X1, nullptr, st))) return rc;
-    if ((rc = linear<FMT>(e->X1, H, Mr, d.w1, F, H, d.b1, nullptr, gelu_form(), e->FF, nullptr, st, ance::kClsGemmFfn1))) return rc;
-    if ((rc = linear<FMT>(e->FF, F, Mr, d.w2, H, F, d.b2, e->X1, 0, e->T, nullptr, st, ance::kClsGemmFfn2))) return rc;
-    if ((rc = layer_norm<FMT>(e->T, false, H, Mr, H, d.ln2g, d.ln2b, c.ln_eps, e->X, nullptr, st))) return rc;
+    if ((rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch))) return rc;
+    if ((rc = layer_norm<FMT>(T1, false, H, Mr, H, d.ln1g, d.ln1b, c.ln_eps, X1, nullptr, st))) return rc;
+    if (ts && (rc = linear<FMT>(X1, H, Mr, d.w1, F, H, d.b1, nullptr, 0, ts->at(l, ts->lo.u), nullptr, st, ance::kClsGemmFfn1))) return rc;
+    if ((rc = linear<FMT>(X1, H, Mr, d.w1, F, H, d.b1, nullptr, gelu_form(), FF, nullptr, st, ance::kClsGemmFfn1))) return rc;
+    if ((rc = linear<FMT>(FF, F, Mr, d.w2, H, F, d.b2, X1, 0, T2, nullptr, st, ance::kClsGemmFfn2))) return rc;
+    if ((rc = layer_norm<FMT>(T2, false, H, Mr, H, d.ln2g, d.ln2b, c.ln_eps, X_out, nullptr, st))) return rc;
     if (e->dbg && M <= e->dbg_tokens)  // with cls_only the first B rows hold the CLS rows of the last layer
-      ANCE_CUDA(cudaMemcpyAsync(e->dbg + static_cast<size_t>(l + 1) * e->dbg_tokens * H, e->X, static_cast<size_t>(Mr) * H * 2, cudaMemcpyDeviceToDevice, st));
+      ANCE_CUDA(cudaMemcpyAsync(e->dbg + static_cast<size_t>(l + 1) * e->dbg_tokens * H, X_out, static_cast<size_t>(Mr) * H * 2, cudaMemcpyDeviceToDevice, st));
   }
-  const size_t cls_pitch = (e->prune_last_layer || varlen) ? static_cast<size_t>(H) : static_cast<size_t>(L) * H;
+  const size_t cls_pitch = (e->prune_last_layer || varlen || ts) ? static_cast<size_t>(H) : static_cast<size_t>(L) * H;
+  const uint16_t* X_last = ts ? ts->x(c.n_layer) : e->X;
   // K7: CLS rows (token 0 of every sequence) -> head
   if (c.has_head) {
     // A = the CLS rows of X ([B, H] compact after the pruned last layer, else row pitch L*H)
-    if ((rc = linear<FMT>(e->X, cls_pitch, B, e->head_w, H, H, e->head_b, nullptr, 0, nullptr, e->head_tmp, st))) return rc;
-    if ((rc = layer_norm<FMT>(e->head_tmp, true, H, B, H, e->head_g, e->head_bt, 1e-5f, nullptr, out_dev, st))) return rc;
+    float* head_in = ts ? ts->head_in() : e->head_tmp;
+    if ((rc = linear<FMT>(X_last, cls_pitch, B, e->head_w, H, H, e->head_b, nullptr, 0, nullptr, head_in, st))) return rc;
+    if ((rc = layer_norm<FMT>(head_in, true, H, B, H, e->head_g, e->head_bt, 1e-5f, nullptr, out_dev, st))) return rc;
   } else {
     ance::ProfScope ps(ance::kClsNorm, st);
-    gather_rows_f32_kernel<FMT><<<B, 256, 0, st>>>(e->X, cls_pitch, B, H, out_dev);
+    gather_rows_f32_kernel<FMT><<<B, 256, 0, st>>>(X_last, cls_pitch, B, H, out_dev);
     ANCE_CUDA(cudaGetLastError());
     ance::count_launch(1);
   }
@@ -792,6 +865,8 @@ extern "C" int ance_encoder_create(const ance_encoder_config* cfg, const ance_en
 extern "C" int ance_encoder_destroy(ance_encoder_t e) {
   if (!e) return ANCE_OK;
   for (void* p : e->allocs) cudaFree(p);
+  if (e->bwd_scratch) cudaFree(e->bwd_scratch);
+  if (e->refresh_dev) cudaFree(e->refresh_dev);
   delete e;
   return ANCE_OK;
 }
@@ -814,6 +889,416 @@ extern "C" int ance_encoder_forward(ance_encoder_t e, const int32_t* ids_dev, co
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st);
   return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st);
+}
+
+// ------------------------------------------------------------------------------------------------
+// training: forward with saved activations, backward, in-place weight refresh
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr uint32_t kBF = tc05::kFmtBF16;   // every backward GEMM runs on bf16 operands (gradients can underflow fp16)
+
+unsigned ew_grid(size_t n) { return static_cast<unsigned>(std::min<size_t>((n + 255) / 256, 8192)); }
+
+// dst [C, dst_ld] bf16 = src[R, C]^T (kSrc 0 fp16, 1 bf16, 2 fp32), columns R .. dst_ld - 1 zero
+template <int kSrc>
+int transpose_bf16(const void* src, size_t src_ld, int R, int C, uint16_t* dst, size_t dst_ld, cudaStream_t st) {
+  const dim3 grid(static_cast<unsigned>((dst_ld + 31) / 32), static_cast<unsigned>((C + 31) / 32));
+  bwd::transpose_bf16_kernel<kSrc><<<grid, dim3(32, 8), 0, st>>>(src, src_ld, R, C, dst, dst_ld);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+template <uint32_t FMT>
+constexpr int src_code() { return FMT == tc05::kFmtBF16 ? 1 : 0; }
+
+int to_bf16(const float* a, uint16_t* o, size_t n, cudaStream_t st) {
+  bwd::f32_to_bf16_kernel<<<ew_grid(n), 256, 0, st>>>(a, o, n);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+int add_rows(float* dst, size_t dst_row_stride, const float* src, int rows, int H, cudaStream_t st) {
+  bwd::add_rows_kernel<<<ew_grid(static_cast<size_t>(rows) * H), 256, 0, st>>>(dst, dst_row_stride, src, rows, H);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+// column sums of fp32 a [rows, N] -> o0 / o1 / o2 (segments of `seg` columns), deterministic
+int colsum(const float* a, int rows, int N, float* part, int seg, float* o0, float* o1, float* o2, cudaStream_t st) {
+  int chunks = std::min(rows, bwd::kColsumChunks);
+  const int per = (rows + chunks - 1) / chunks;
+  chunks = (rows + per - 1) / per;
+  bwd::colsum_partial_kernel<<<dim3((N + 255) / 256, chunks), 256, 0, st>>>(a, rows, N, per, part);
+  bwd::colsum_final_kernel<<<(N + 255) / 256, 256, 0, st>>>(part, chunks, N, seg, o0, o1, o2);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(2);
+  return ANCE_OK;
+}
+
+// LayerNorm backward of `rows` rows + dgamma / dbeta / dbias (any of the three may be null); part: scratch of
+// kLnBwdMaxBlocks * 3H floats
+template <uint32_t FMT>
+int ln_bwd(const void* x, bool in_f32, size_t x_ld, int rows, int H, const float* gamma, float eps, const float* dy,
+           float* dx, float* part, float* dgamma, float* dbeta, float* dbias, cudaStream_t st) {
+  const int blocks = std::min((rows + 7) / 8, bwd::kLnBwdMaxBlocks);
+  ance::ProfScope ps(ance::kClsNorm, st);
+#define LNB_CASE(NV_)                                                                                                  \
+  if (in_f32) bwd::ln_bwd_kernel<NV_, true, FMT><<<blocks, 256, 0, st>>>(x, x_ld, rows, H, gamma, eps, dy, dx, part);   \
+  else bwd::ln_bwd_kernel<NV_, false, FMT><<<blocks, 256, 0, st>>>(x, x_ld, rows, H, gamma, eps, dy, dx, part)
+  switch (H / 256) {
+    case 1: LNB_CASE(1); break;
+    case 2: LNB_CASE(2); break;
+    case 3: LNB_CASE(3); break;
+    case 4: LNB_CASE(4); break;
+    default: ance::set_error("encoder backward: hidden size %d unsupported", H); return ANCE_ERR_UNSUPPORTED;
+  }
+#undef LNB_CASE
+  bwd::colsum_final_kernel<<<(3 * H + 255) / 256, 256, 0, st>>>(part, blocks, 3 * H, H, dgamma, dbeta, dbias);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(2);
+  return ANCE_OK;
+}
+
+template <uint32_t FMT>
+int attn_bwd(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, int B, int L,
+             int heads, cudaStream_t st) {
+  const size_t smem = bwd::attn_bwd_smem(L);
+  ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
+  ance::ProfScope ps(ance::kClsAttn, st);
+  bwd::attn_bwd_kernel<FMT><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+// bf16 W^T copies of every linear weight (dgrad operands), rebuilt from the 16-bit weights after a change
+template <uint32_t FMT>
+int ensure_wt(ance_encoder* e, cudaStream_t st) {
+  const ance_encoder_config& c = e->cfg;
+  const size_t H = c.hidden, F = c.ffn;
+  if (e->wt.empty()) {
+    std::vector<ance_encoder::LayerT> wt(c.n_layer);
+    bool ok = true;
+    for (auto& t : wt) {
+      ok = ok && (t.wqkv = dev_alloc<uint16_t>(e, 3 * H * H)) && (t.wo = dev_alloc<uint16_t>(e, H * H)) &&
+           (t.w1 = dev_alloc<uint16_t>(e, F * H)) && (t.w2 = dev_alloc<uint16_t>(e, H * F));
+    }
+    if (c.has_head) ok = ok && (e->head_wt = dev_alloc<uint16_t>(e, H * H));
+    if (!ok) {
+      ance::set_error("encoder backward: allocating the transposed weights failed");
+      return ANCE_ERR_NOMEM;
+    }
+    e->wt = wt;
+    e->wt_stale = true;
+  }
+  if (!e->wt_stale) return ANCE_OK;
+  constexpr int S = src_code<FMT>();
+  int rc;
+  for (int l = 0; l < c.n_layer; ++l) {
+    const LayerDev& d = e->layers[l];
+    const ance_encoder::LayerT& t = e->wt[l];
+    if ((rc = transpose_bf16<S>(d.wqkv, H, 3 * H, H, t.wqkv, 3 * H, st))) return rc;
+    if ((rc = transpose_bf16<S>(d.wo, H, H, H, t.wo, H, st))) return rc;
+    if ((rc = transpose_bf16<S>(d.w1, H, F, H, t.w1, F, st))) return rc;
+    if ((rc = transpose_bf16<S>(d.w2, F, H, F, t.w2, H, st))) return rc;
+  }
+  if (c.has_head && (rc = transpose_bf16<S>(e->head_w, H, H, H, e->head_wt, H, st))) return rc;
+  e->wt_stale = false;
+  return ANCE_OK;
+}
+
+struct BwdScratch {
+  float *G, *dT, *dA, *dX1, *part;
+  uint16_t *A16, *Gt, *Xt, *dCTX;
+  int32_t* pos;
+};
+
+int ensure_scratch(ance_encoder* e, int M, BwdScratch& s) {
+  const size_t H = e->cfg.hidden, F = e->cfg.ffn, N = std::max(3 * H, F), Mp = (M + 7) / 8 * 8;
+  auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t part = std::max(static_cast<size_t>(bwd::kLnBwdMaxBlocks) * 3 * H, static_cast<size_t>(bwd::kColsumChunks) * N);
+  const size_t sz[10] = {up(M * H * 4), up(M * H * 4), up(M * N * 4), up(M * H * 4), up(part * 4),
+                         up(M * N * 2), up(N * Mp * 2), up(N * Mp * 2), up(M * H * 2), up(static_cast<size_t>(M) * 4)};
+  size_t total = 0;
+  for (size_t x : sz) total += x;
+  if (total > e->bwd_scratch_bytes) {
+    if (e->bwd_scratch) cudaFree(e->bwd_scratch);
+    e->bwd_scratch = nullptr;
+    e->bwd_scratch_bytes = 0;
+    if (cudaMalloc(&e->bwd_scratch, total) != cudaSuccess) {
+      e->bwd_scratch = nullptr;
+      ance::set_error("encoder backward: allocating %zu bytes of scratch failed", total);
+      return ANCE_ERR_NOMEM;
+    }
+    e->bwd_scratch_bytes = total;
+  }
+  uint8_t* p = reinterpret_cast<uint8_t*>(e->bwd_scratch);
+  void* q[10];
+  for (int i = 0; i < 10; ++i) { q[i] = p; p += sz[i]; }
+  s.G = static_cast<float*>(q[0]); s.dT = static_cast<float*>(q[1]); s.dA = static_cast<float*>(q[2]);
+  s.dX1 = static_cast<float*>(q[3]); s.part = static_cast<float*>(q[4]);
+  s.A16 = static_cast<uint16_t*>(q[5]); s.Gt = static_cast<uint16_t*>(q[6]); s.Xt = static_cast<uint16_t*>(q[7]);
+  s.dCTX = static_cast<uint16_t*>(q[8]); s.pos = static_cast<int32_t*>(q[9]);
+  return ANCE_OK;
+}
+
+// C32 [N_out, K_in] = dY^T X over `rows` tokens: A = dY^T [N_out, rows_p] and W = X^T [K_in, rows_p] (bf16, zero columns
+// past `rows`, so K = rows_p is exact)
+int wgrad(const uint16_t* dYt, int n_out, const uint16_t* Xt, int k_in, int rows_p, float* C32, cudaStream_t st) {
+  return linear<kBF>(dYt, rows_p, n_out, Xt, k_in, rows_p, nullptr, nullptr, 0, nullptr, C32, st);
+}
+
+template <uint32_t FMT>
+int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws, const ance_encoder_grads* g,
+                  cudaStream_t st) {
+  const ance_encoder_config& c = e->cfg;
+  const int H = c.hidden, F = c.ffn, M = B * L, Mp = (M + 7) / 8 * 8, NL = c.n_layer;
+  constexpr int S = src_code<FMT>();
+  TrainSave ts{ws, train_layout(c, B, L), NL};
+  BwdScratch s;
+  int rc;
+  if ((rc = ensure_wt<FMT>(e, st))) return rc;
+  if ((rc = ensure_scratch(e, M, s))) return rc;
+  const int Bp = (B + 7) / 8 * 8;
+  // head: out = LN(X_cls Wh^T + bh) -> s.G = d X_cls [B, H]
+  if (c.has_head) {
+    if ((rc = ln_bwd<FMT>(ts.head_in(), true, H, B, H, e->head_g, 1e-5f, d_out, s.dT, s.part, g->head_ln_g, g->head_ln_b, g->head_b, st))) return rc;
+    if ((rc = to_bf16(s.dT, s.A16, static_cast<size_t>(B) * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(s.dT, H, B, H, s.Gt, Bp, st))) return rc;
+    if ((rc = transpose_bf16<S>(ts.x(NL), H, B, H, s.Xt, Bp, st))) return rc;
+    if ((rc = wgrad(s.Gt, H, s.Xt, H, Bp, g->head_w, st))) return rc;
+    if ((rc = linear<kBF>(s.A16, H, B, e->head_wt, H, H, nullptr, nullptr, 0, nullptr, s.G, st))) return rc;
+  } else {
+    ANCE_CUDA(cudaMemcpyAsync(s.G, d_out, static_cast<size_t>(B) * H * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  for (int l = NL - 1; l >= 0; --l) {
+    const LayerDev& d = e->layers[l];
+    const ance_encoder::LayerT& wt = e->wt[l];
+    const ance_layer_grads& lg = g->layers[l];
+    const bool last = l == NL - 1;
+    const int Mr = last ? B : M, Mrp = (Mr + 7) / 8 * 8;
+    // s.G = d X_out [Mr, H].  LN2: T2 = FF W2^T + b2 + X1
+    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t2), false, H, Mr, H, d.ln2g, c.ln_eps, s.G, s.dT, s.part, lg.ln2_g, lg.ln2_b, lg.ff2_b, st))) return rc;
+    if ((rc = to_bf16(s.dT, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(s.dT, H, Mr, H, s.Gt, Mrp, st))) return rc;
+    if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.ff), F, Mr, F, s.Xt, Mrp, st))) return rc;
+    if ((rc = wgrad(s.Gt, H, s.Xt, F, Mrp, lg.ff2_w, st))) return rc;
+    if ((rc = linear<kBF>(s.A16, H, Mr, wt.w2, F, H, nullptr, nullptr, 0, nullptr, s.dA, st))) return rc;   // d FF
+    {
+      const size_t n = static_cast<size_t>(Mr) * F;
+      bwd::gelu_bwd_kernel<FMT><<<ew_grid(n), 256, 0, st>>>(ts.at(l, ts.lo.u), s.dA, n);   // d U
+      ANCE_CUDA(cudaGetLastError());
+      ance::count_launch(1);
+    }
+    if ((rc = colsum(s.dA, Mr, F, s.part, F, lg.ff1_b, nullptr, nullptr, st))) return rc;
+    if ((rc = to_bf16(s.dA, s.A16, static_cast<size_t>(Mr) * F, st))) return rc;
+    if ((rc = transpose_bf16<2>(s.dA, F, Mr, F, s.Gt, Mrp, st))) return rc;
+    if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.x1), H, Mr, H, s.Xt, Mrp, st))) return rc;
+    if ((rc = wgrad(s.Gt, F, s.Xt, H, Mrp, lg.ff1_w, st))) return rc;
+    if ((rc = linear<kBF>(s.A16, F, Mr, wt.w1, H, F, nullptr, nullptr, 0, nullptr, s.dX1, st))) return rc;   // d X1 (FFN)
+    if ((rc = add_rows(s.dX1, 1, s.dT, Mr, H, st))) return rc;                                              // + residual
+    // LN1: T1 = CTX Wo^T + bo + X_in
+    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t1), false, H, Mr, H, d.ln1g, c.ln_eps, s.dX1, s.dT, s.part, lg.ln1_g, lg.ln1_b, lg.ao_b, st))) return rc;
+    if ((rc = to_bf16(s.dT, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(s.dT, H, Mr, H, s.Gt, Mrp, st))) return rc;
+    if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.ctx), last ? static_cast<size_t>(L) * H : H, Mr, H, s.Xt, Mrp, st))) return rc;
+    if ((rc = wgrad(s.Gt, H, s.Xt, H, Mrp, lg.ao_w, st))) return rc;
+    if ((rc = linear<kBF>(s.A16, H, Mr, wt.wo, H, H, nullptr, nullptr, 0, s.dCTX, nullptr, st))) return rc;  // d CTX (bf16)
+    // attention -> d QKV [M, 3H]
+    if ((rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st))) return rc;
+    if ((rc = colsum(s.dA, M, 3 * H, s.part, H, lg.q_b, lg.k_b, lg.v_b, st))) return rc;
+    if ((rc = to_bf16(s.dA, s.A16, static_cast<size_t>(M) * 3 * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(s.dA, 3 * H, M, 3 * H, s.Gt, Mp, st))) return rc;
+    if ((rc = transpose_bf16<S>(ts.x(l), H, M, H, s.Xt, Mp, st))) return rc;
+    float* const wq[3] = {lg.q_w, lg.k_w, lg.v_w};
+    for (int p = 0; p < 3; ++p)
+      if ((rc = wgrad(s.Gt + static_cast<size_t>(p) * H * Mp, H, s.Xt, H, Mp, wq[p], st))) return rc;
+    if ((rc = linear<kBF>(s.A16, 3 * H, M, wt.wqkv, H, 3 * H, nullptr, nullptr, 0, nullptr, s.G, st))) return rc;   // d X_in
+    if ((rc = add_rows(s.G, last ? L : 1, s.dT, Mr, H, st))) return rc;   // + residual (the CLS rows in the last layer)
+  }
+  // embeddings: X0 = LN((word[id] + pos[p]) + type[0])
+  {
+    ance::ProfScope ps(ance::kClsNorm, st);
+    bwd::embed_sum_kernel<<<B, 256, 0, st>>>(ts.ids(), L, H, c.arch == ANCE_ARCH_ROBERTA, c.pad_id, c.vocab, c.max_pos,
+                                             e->word, e->pos, e->type, s.dA, s.pos);
+    ANCE_CUDA(cudaGetLastError());
+    ance::count_launch(1);
+  }
+  ANCE_CUDA(cudaMemsetAsync(g->word_emb, 0, static_cast<size_t>(c.vocab) * H * 4, st));
+  ANCE_CUDA(cudaMemsetAsync(g->pos_emb, 0, static_cast<size_t>(c.max_pos) * H * 4, st));
+  ANCE_CUDA(cudaMemsetAsync(g->type_emb, 0, static_cast<size_t>(c.type_vocab) * H * 4, st));
+  if ((rc = ln_bwd<FMT>(s.dA, true, H, M, H, e->eg, c.ln_eps, s.G, s.dT, s.part, g->emb_ln_g, g->emb_ln_b, g->type_emb, st))) return rc;
+  {
+    ance::ProfScope ps(ance::kClsNorm, st);
+    bwd::embed_scatter_kernel<<<M, 256, 0, st>>>(ts.ids(), s.pos, s.dT, M, H, c.arch == ANCE_ARCH_ROBERTA, c.pad_id, c.vocab,
+                                                 g->word_emb, g->pos_emb);
+    ANCE_CUDA(cudaGetLastError());
+    ance::count_launch(1);
+  }
+  return ANCE_OK;
+}
+
+// One launch converts every parameter into the handle: a table of (source, destination, count, kind) pieces of at most
+// bwd::kRefreshChunk elements, one block each.  The table is re-uploaded only when a pointer changed.
+template <uint32_t FMT>
+int update_weights_impl(ance_encoder* e, const ance_encoder_weights* w, cudaStream_t st) {
+  const ance_encoder_config& c = e->cfg;
+  const size_t H = c.hidden, F = c.ffn;
+  std::vector<bwd::RefreshPiece> t;
+  auto add = [&](const float* src, void* dst, size_t n, uint32_t to16) {
+    for (size_t o = 0; o < n; o += bwd::kRefreshChunk) {
+      bwd::RefreshPiece r;
+      r.src = src + o;
+      r.dst = to16 ? static_cast<void*>(static_cast<uint16_t*>(dst) + o) : static_cast<void*>(static_cast<float*>(dst) + o);
+      r.n = static_cast<uint32_t>(std::min<size_t>(bwd::kRefreshChunk, n - o));
+      r.to16 = to16;
+      t.push_back(r);
+    }
+  };
+  add(w->word_emb, e->word, static_cast<size_t>(c.vocab) * H, 0);
+  add(w->pos_emb, e->pos, static_cast<size_t>(c.max_pos) * H, 0);
+  add(w->type_emb, e->type, static_cast<size_t>(c.type_vocab) * H, 0);
+  add(w->emb_ln_g, e->eg, H, 0);
+  add(w->emb_ln_b, e->eb, H, 0);
+  for (int l = 0; l < c.n_layer; ++l) {
+    const ance_layer_weights& lw = w->layers[l];
+    const LayerDev& d = e->layers[l];
+    add(lw.q_w, d.wqkv, H * H, 1);
+    add(lw.k_w, d.wqkv + H * H, H * H, 1);
+    add(lw.v_w, d.wqkv + 2 * H * H, H * H, 1);
+    add(lw.q_b, d.bqkv, H, 0);
+    add(lw.k_b, d.bqkv + H, H, 0);
+    add(lw.v_b, d.bqkv + 2 * H, H, 0);
+    add(lw.ao_w, d.wo, H * H, 1);
+    add(lw.ao_b, d.bo, H, 0);
+    add(lw.ln1_g, d.ln1g, H, 0);
+    add(lw.ln1_b, d.ln1b, H, 0);
+    add(lw.ff1_w, d.w1, F * H, 1);
+    add(lw.ff1_b, d.b1, F, 0);
+    add(lw.ff2_w, d.w2, H * F, 1);
+    add(lw.ff2_b, d.b2, H, 0);
+    add(lw.ln2_g, d.ln2g, H, 0);
+    add(lw.ln2_b, d.ln2b, H, 0);
+  }
+  if (c.has_head) {
+    add(w->head_w, e->head_w, H * H, 1);
+    add(w->head_b, e->head_b, H, 0);
+    add(w->head_ln_g, e->head_g, H, 0);
+    add(w->head_ln_b, e->head_bt, H, 0);
+  }
+  const size_t bytes = t.size() * sizeof(bwd::RefreshPiece);
+  const bool same = e->refresh_table.size() == t.size() && memcmp(e->refresh_table.data(), t.data(), bytes) == 0;
+  if (!same) {
+    if (t.size() > e->refresh_cap) {   // grows once; the old table is freed after the work queued before it
+      if (e->refresh_dev) ANCE_CUDA(cudaFreeAsync(e->refresh_dev, st));
+      e->refresh_dev = nullptr;
+      e->refresh_cap = 0;
+      ANCE_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&e->refresh_dev), bytes, st));
+      e->refresh_cap = t.size();
+    }
+    e->refresh_table = t;   // kept alive: the pageable copy below reads it
+    ANCE_CUDA(cudaMemcpyAsync(e->refresh_dev, e->refresh_table.data(), bytes, cudaMemcpyHostToDevice, st));
+  }
+  bwd::refresh_kernel<FMT><<<static_cast<unsigned>(t.size()), 256, 0, st>>>(e->refresh_dev);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  e->wt_stale = true;
+  return ANCE_OK;
+}
+
+// ance_encoder_grads is ance_encoder_weights with writable pointers: the same checks serve both
+static_assert(sizeof(ance_layer_grads) == sizeof(ance_layer_weights) && sizeof(ance_encoder_grads) == sizeof(ance_encoder_weights),
+              "gradient and weight structs must share one layout");
+
+// every pointer the config needs is non-null (and, with `aligned`, 16-byte aligned: the kernels use 16-byte accesses)
+bool weights_complete(const ance_encoder_config& c, const ance_encoder_weights* w, bool aligned = false) {
+  auto ok = [&](const void* q) { return q && (!aligned || (reinterpret_cast<uintptr_t>(q) & 15u) == 0); };
+  if (!ok(w->word_emb) || !ok(w->pos_emb) || !ok(w->type_emb) || !ok(w->emb_ln_g) || !ok(w->emb_ln_b) || !w->layers) return false;
+  for (int l = 0; l < c.n_layer; ++l) {
+    const ance_layer_weights& x = w->layers[l];
+    const float* const p[16] = {x.q_w, x.q_b, x.k_w, x.k_b, x.v_w, x.v_b, x.ao_w, x.ao_b, x.ln1_g, x.ln1_b,
+                                x.ff1_w, x.ff1_b, x.ff2_w, x.ff2_b, x.ln2_g, x.ln2_b};
+    for (const float* q : p)
+      if (!ok(q)) return false;
+  }
+  return !c.has_head || (ok(w->head_w) && ok(w->head_b) && ok(w->head_ln_g) && ok(w->head_ln_b));
+}
+
+}  // namespace
+
+extern "C" int ance_encoder_train_workspace(ance_encoder_t e, int B, int L, size_t* bytes) {
+  ANCE_REQUIRE(e != nullptr && bytes != nullptr, "ance_encoder_train_workspace: null argument");
+  ANCE_REQUIRE(B > 0 && L > 0, "ance_encoder_train_workspace: empty batch");
+  if (L > attn::kTile) {
+    ance::set_error("ance_encoder_train_workspace: L = %d; the backward covers sequences of up to 128 tokens", L);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  *bytes = train_layout(e->cfg, B, L).total;
+  return ANCE_OK;
+}
+
+extern "C" int ance_encoder_forward_train(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
+                                          const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev, void* stream) {
+  ANCE_REQUIRE(e != nullptr, "ance_encoder_forward_train: null handle");
+  ANCE_REQUIRE(ids_dev && out_dev && ws_dev, "ance_encoder_forward_train: null buffer");
+  ANCE_REQUIRE((lens_dev != nullptr) != (mask_dev != nullptr), "ance_encoder_forward_train: pass exactly one of lens_dev / mask_dev");
+  ANCE_REQUIRE(B > 0 && L > 0, "ance_encoder_forward_train: empty batch");
+  if (L > attn::kTile) {
+    ance::set_error("ance_encoder_forward_train: L = %d; the backward covers sequences of up to 128 tokens", L);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  ANCE_REQUIRE(128 % L == 0 && L >= 8, "ance_encoder_forward_train: L = %d unsupported (need a divisor of 128, >= 8)", L);
+  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(ws_dev) & 255u) == 0, "ance_encoder_forward_train: the workspace must be 256-byte aligned");
+  const ance_encoder_config& c = e->cfg;
+  ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "ance_encoder_forward_train: L = %d exceeds max_position_embeddings %d", L, c.max_pos);
+  const long long tokens = static_cast<long long>(B) * L;
+  ANCE_REQUIRE(tokens <= e->max_tokens, "ance_encoder_forward_train: %lld tokens exceed max_tokens %d", tokens, e->max_tokens);
+  ANCE_REQUIRE(B <= e->max_tokens / 16, "ance_encoder_forward_train: batch %d too large for the head buffer", B);
+  int dev = -1;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  ANCE_REQUIRE(dev == e->device, "ance_encoder_forward_train: the handle belongs to device %d but device %d is current", e->device, dev);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const TrainSave ts{reinterpret_cast<uint8_t*>(ws_dev), train_layout(c, B, L), c.n_layer};
+  e->train_shapes[ws_dev] = make_int2(B, L);
+  if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts);
+  return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts);
+}
+
+extern "C" int ance_encoder_backward(ance_encoder_t e, const float* d_out_dev, void* ws_dev, const ance_encoder_grads* g,
+                                     void* stream) {
+  ANCE_REQUIRE(e != nullptr, "ance_encoder_backward: null handle");
+  ANCE_REQUIRE(d_out_dev && ws_dev && g, "ance_encoder_backward: null argument");
+  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(d_out_dev) & 15u) == 0, "ance_encoder_backward: d_out must be 16-byte aligned");
+  const auto it = e->train_shapes.find(ws_dev);
+  ANCE_REQUIRE(it != e->train_shapes.end(), "ance_encoder_backward: the workspace was not filled by ance_encoder_forward_train on "
+               "this handle, or its backward has already run");
+  const ance_encoder_config& c = e->cfg;
+  ANCE_REQUIRE(weights_complete(c, reinterpret_cast<const ance_encoder_weights*>(g), true),
+               "ance_encoder_backward: a gradient pointer is null or not 16-byte aligned");
+  int dev = -1;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  ANCE_REQUIRE(dev == e->device, "ance_encoder_backward: the handle belongs to device %d but device %d is current", e->device, dev);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  auto* ws = reinterpret_cast<uint8_t*>(ws_dev);
+  const int2 shape = it->second;
+  e->train_shapes.erase(it);   // one backward per forward_train: the record cannot outlive the caller's workspace
+  if (e->fmt == tc05::kFmtBF16) return backward_impl<tc05::kFmtBF16>(e, shape.x, shape.y, d_out_dev, ws, g, st);
+  return backward_impl<tc05::kFmtF16>(e, shape.x, shape.y, d_out_dev, ws, g, st);
+}
+
+extern "C" int ance_encoder_update_weights(ance_encoder_t e, const ance_encoder_weights* w_dev, void* stream) {
+  ANCE_REQUIRE(e != nullptr && w_dev != nullptr, "ance_encoder_update_weights: null argument");
+  ANCE_REQUIRE(weights_complete(e->cfg, w_dev), "ance_encoder_update_weights: a weight pointer is null");
+  int dev = -1;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  ANCE_REQUIRE(dev == e->device, "ance_encoder_update_weights: the handle belongs to device %d but device %d is current", e->device, dev);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->fmt == tc05::kFmtBF16) return update_weights_impl<tc05::kFmtBF16>(e, w_dev, st);
+  return update_weights_impl<tc05::kFmtF16>(e, w_dev, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1156,4 +1641,89 @@ extern "C" int ance_dbg_layer_norm(int fmt, const void* in_dev, int in_f32, int6
                                                  reinterpret_cast<uint16_t*>(out16_dev), out32_dev, st);
   g_ln_rows_per_warp = saved;
   return rc;
+}
+
+extern "C" int ance_dbg_attention_backward(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                           int cls_only, int B, int L, int heads, float* dqkv_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_attention_backward: unknown operand format %d", fmt);
+  ANCE_REQUIRE(qkv_dev && kbias_dev && dout_bf16_dev && dqkv_dev, "ance_dbg_attention_backward: null buffer");
+  ANCE_REQUIRE(heads >= 1 && heads <= 16, "ance_dbg_attention_backward: heads = %d outside [1, 16]", heads);
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= attn::kTile, "ance_dbg_attention_backward: need B > 0 and 0 < L <= 128 (B = %d, L = %d)", B, L);
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* qkv = reinterpret_cast<const uint16_t*>(qkv_dev);
+  const auto* dout = reinterpret_cast<const uint16_t*>(dout_bf16_dev);
+  if (fmt == ANCE_FMT_BF16) return attn_bwd<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st);
+  return attn_bwd<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st);
+}
+
+extern "C" int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
+                                            const float* gamma_dev, float eps, const float* dy_dev, float* dx_dev,
+                                            float* dgamma_dev, float* dbeta_dev, float* dsum_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_layer_norm_backward: unknown operand format %d", fmt);
+  ANCE_REQUIRE(in_dev && gamma_dev && dy_dev && dx_dev, "ance_dbg_layer_norm_backward: null buffer");
+  ANCE_REQUIRE(rows > 0 && H > 0 && H % 256 == 0 && H <= 1024, "ance_dbg_layer_norm_backward: need rows > 0 and H in {256, 512, 768, 1024} (rows = %d, H = %d)", rows, H);
+  ANCE_REQUIRE(in_ld >= H && in_ld % 8 == 0, "ance_dbg_layer_norm_backward: in_ld = %lld must be >= H and a multiple of 8", static_cast<long long>(in_ld));
+  ANCE_REQUIRE(aligned16(in_dev) && aligned16(gamma_dev) && aligned16(dy_dev) && aligned16(dx_dev),
+               "ance_dbg_layer_norm_backward: every buffer must be 16-byte aligned");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* part = nullptr;
+  ANCE_CUDA(cudaMallocAsync(&part, static_cast<size_t>(bwd::kLnBwdMaxBlocks) * 3 * H * 4, st));
+  const int rc = (fmt == ANCE_FMT_BF16)
+                     ? ln_bwd<tc05::kFmtBF16>(in_dev, in_f32 != 0, static_cast<size_t>(in_ld), rows, H, gamma_dev, eps, dy_dev, dx_dev, part, dgamma_dev, dbeta_dev, dsum_dev, st)
+                     : ln_bwd<tc05::kFmtF16>(in_dev, in_f32 != 0, static_cast<size_t>(in_ld), rows, H, gamma_dev, eps, dy_dev, dx_dev, part, dgamma_dev, dbeta_dev, dsum_dev, st);
+  ANCE_CUDA(cudaFreeAsync(part, st));
+  return rc;
+}
+
+extern "C" int ance_dbg_gelu_backward(int fmt, const void* u_dev, float* g_dev, int64_t n, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_gelu_backward: unknown operand format %d", fmt);
+  ANCE_REQUIRE(u_dev && g_dev && n > 0, "ance_dbg_gelu_backward: null buffer or n <= 0");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* u = reinterpret_cast<const uint16_t*>(u_dev);
+  if (fmt == ANCE_FMT_BF16) bwd::gelu_bwd_kernel<tc05::kFmtBF16><<<ew_grid(n), 256, 0, st>>>(u, g_dev, static_cast<size_t>(n));
+  else bwd::gelu_bwd_kernel<tc05::kFmtF16><<<ew_grid(n), 256, 0, st>>>(u, g_dev, static_cast<size_t>(n));
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+extern "C" int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int roberta, int pad_id, int vocab,
+                                           int max_pos, const float* word_dev, const float* pos_dev, const float* type_dev,
+                                           const float* dE_dev, float* E_dev, float* dword_dev, float* dpos_dev,
+                                           void* stream) {
+  ANCE_REQUIRE(ids_dev && word_dev && pos_dev && type_dev && dE_dev && E_dev && dword_dev && dpos_dev,
+               "ance_dbg_embedding_backward: null buffer");
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= attn::kTile && H > 0 && vocab > 0 && max_pos > 0,
+               "ance_dbg_embedding_backward: need B, H, vocab, max_pos > 0 and 0 < L <= 128 (B = %d, L = %d)", B, L);
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int M = B * L;
+  int32_t* pos_ids = nullptr;
+  ANCE_CUDA(cudaMallocAsync(&pos_ids, static_cast<size_t>(M) * 4, st));
+  bwd::embed_sum_kernel<<<B, 256, 0, st>>>(ids_dev, L, H, roberta != 0, pad_id, vocab, max_pos, word_dev, pos_dev, type_dev,
+                                           E_dev, pos_ids);
+  ANCE_CUDA(cudaMemsetAsync(dword_dev, 0, static_cast<size_t>(vocab) * H * 4, st));
+  ANCE_CUDA(cudaMemsetAsync(dpos_dev, 0, static_cast<size_t>(max_pos) * H * 4, st));
+  bwd::embed_scatter_kernel<<<M, 256, 0, st>>>(ids_dev, pos_ids, dE_dev, M, H, roberta != 0, pad_id, vocab, dword_dev, dpos_dev);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(2);
+  ANCE_CUDA(cudaFreeAsync(pos_ids, st));
+  return ANCE_OK;
+}
+
+extern "C" int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, int R, int C, void* dst_dev,
+                                       int64_t dst_ld, void* stream) {
+  ANCE_REQUIRE(src_kind >= 0 && src_kind <= 2, "ance_dbg_transpose_bf16: src_kind must be 0 (fp16), 1 (bf16) or 2 (fp32), got %d", src_kind);
+  ANCE_REQUIRE(src_dev && dst_dev, "ance_dbg_transpose_bf16: null buffer");
+  ANCE_REQUIRE(R > 0 && C > 0 && src_ld >= C && dst_ld >= R, "ance_dbg_transpose_bf16: need R, C > 0, src_ld >= C, dst_ld >= R");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t sl = static_cast<size_t>(src_ld), dl = static_cast<size_t>(dst_ld);
+  auto* dst = reinterpret_cast<uint16_t*>(dst_dev);
+  if (src_kind == 2) return transpose_bf16<2>(src_dev, sl, R, C, dst, dl, st);
+  if (src_kind == 1) return transpose_bf16<1>(src_dev, sl, R, C, dst, dl, st);
+  return transpose_bf16<0>(src_dev, sl, R, C, dst, dl, st);
 }

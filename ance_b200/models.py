@@ -11,10 +11,13 @@ The classes are ``nn.Module``s whose parameters carry the checkpoint's own key n
 so ``load_state_dict`` / ``.to(device)`` / DDP wrapping behave as with the reference; the forward
 is NOT PyTorch: ``query_emb`` / ``body_emb`` run the hand-written sm_90a encoder of
 libance_b200.so (csrc/encoder.cu).  There is no CPU path — calling them with CPU tensors raises.
-The training ``forward()`` losses (models.py:58-134,260-271) are out of scope for this package.
+Training: after ``model.set_trainable(True)`` (rdot_nll, inputs of up to 128 tokens) ``query_emb`` / ``body_emb`` /
+``forward()`` build an autograd graph whose backward runs the encoder's own backward kernels, so ``loss.backward()``
+fills the parameters' ``.grad``; by default the outputs carry no graph.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import json
 import os
@@ -76,6 +79,48 @@ def _np(t: torch.Tensor) -> np.ndarray:
     return np.ascontiguousarray(t.detach().float().cpu().numpy())
 
 
+_EMB_FIELDS = ("word_emb", "pos_emb", "type_emb", "emb_ln_g", "emb_ln_b")
+_HEAD_FIELDS = ("head_w", "head_b", "head_ln_g", "head_ln_b")
+
+
+def _param_groups(backbone: nn.Module, head: Optional[tuple]):
+    """The parameters in the order of ance_encoder_weights: embeddings (5), per layer the 16 of ance_layer_weights, head
+    (4, or none)."""
+    emb = backbone.embeddings
+    embs = [emb.word_embeddings.weight, emb.position_embeddings.weight, emb.token_type_embeddings.weight,
+            emb.LayerNorm.weight, emb.LayerNorm.bias]
+    layers = []
+    for l in backbone.encoder.layer:
+        s, ao = l.attention.self, l.attention.output
+        layers.append([s.query.weight, s.query.bias, s.key.weight, s.key.bias, s.value.weight, s.value.bias,
+                       ao.dense.weight, ao.dense.bias, ao.LayerNorm.weight, ao.LayerNorm.bias,
+                       l.intermediate.dense.weight, l.intermediate.dense.bias,
+                       l.output.dense.weight, l.output.dense.bias, l.output.LayerNorm.weight, l.output.LayerNorm.bias])
+    hd = [] if head is None else [head[0].weight, head[0].bias, head[1].weight, head[1].bias]
+    return embs, layers, hd
+
+
+def _fill(struct_cls, layer_cls, groups, ptr):
+    """ctypes weight / gradient struct over `groups` (see _param_groups); ptr maps a tensor to a float pointer.  Returns
+    (struct, layer array): both must stay alive until the call that reads them returns."""
+    embs, layers, hd = groups
+    lw = (layer_cls * len(layers))()
+    for i, ts in enumerate(layers):
+        for (name, _), t in zip(layer_cls._fields_, ts):
+            setattr(lw[i], name, ptr(t))
+    w = struct_cls()
+    for name, t in zip(_EMB_FIELDS, embs):
+        setattr(w, name, ptr(t))
+    w.layers = lw
+    for name, t in zip(_HEAD_FIELDS, hd):
+        setattr(w, name, ptr(t))
+    return w, lw
+
+
+def _dev_ptr(t: torch.Tensor):
+    return C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_float))
+
+
 class _CudaEncoder:
     """Owns one ance_encoder handle built from a backbone's current parameters."""
 
@@ -108,30 +153,13 @@ class _CudaEncoder:
             keep.append(a)
             return a.ctypes.data_as(C.POINTER(C.c_float))
 
-        lw = (_lib.LayerWeights * len(layers))()
-        for i, l in enumerate(layers):
-            s, ao = l.attention.self, l.attention.output
-            lw[i].q_w, lw[i].q_b = fp(s.query.weight), fp(s.query.bias)
-            lw[i].k_w, lw[i].k_b = fp(s.key.weight), fp(s.key.bias)
-            lw[i].v_w, lw[i].v_b = fp(s.value.weight), fp(s.value.bias)
-            lw[i].ao_w, lw[i].ao_b = fp(ao.dense.weight), fp(ao.dense.bias)
-            lw[i].ln1_g, lw[i].ln1_b = fp(ao.LayerNorm.weight), fp(ao.LayerNorm.bias)
-            lw[i].ff1_w, lw[i].ff1_b = fp(l.intermediate.dense.weight), fp(l.intermediate.dense.bias)
-            lw[i].ff2_w, lw[i].ff2_b = fp(l.output.dense.weight), fp(l.output.dense.bias)
-            lw[i].ln2_g, lw[i].ln2_b = fp(l.output.LayerNorm.weight), fp(l.output.LayerNorm.bias)
-        w = _lib.EncoderWeights()
-        w.word_emb, w.pos_emb, w.type_emb = fp(emb.word_embeddings.weight), fp(emb.position_embeddings.weight), fp(
-            emb.token_type_embeddings.weight)
-        w.emb_ln_g, w.emb_ln_b = fp(emb.LayerNorm.weight), fp(emb.LayerNorm.bias)
-        w.layers = lw
         if head is not None:
             lin, norm = head
             if tuple(lin.weight.shape) != (H, H) or tuple(norm.weight.shape) != (H,):
                 # ance_encoder_create reads a hidden x hidden head: any other shape would be read out of bounds
                 raise _lib.AnceError(f"the CUDA encoder's head must be Linear({H}, {H}) + LayerNorm({H}), got "
                                      f"weight {tuple(lin.weight.shape)}")
-            w.head_w, w.head_b = fp(lin.weight), fp(lin.bias)
-            w.head_ln_g, w.head_ln_b = fp(norm.weight), fp(norm.bias)
+        w, lw = _fill(_lib.EncoderWeights, _lib.LayerWeights, _param_groups(backbone, head), fp)
         self.hidden_size = H
         self.max_tokens = int(max_tokens)
         h = C.c_void_p()
@@ -185,6 +213,67 @@ class _CudaEncoder:
                     None if mask is None else mask[s:e].data_ptr(), e - s, L, out[s:e].data_ptr(), st))
         return out
 
+    def update_weights(self, backbone: nn.Module, head: Optional[tuple]) -> bool:
+        """Refresh the handle in place from the parameters' current values (device fp32, no host round trip); False
+        when a parameter is not a contiguous fp32 tensor on this encoder's device (the caller then rebuilds)."""
+        groups = _param_groups(backbone, head)
+        flat = groups[0] + [t for l in groups[1] for t in l] + groups[2]
+        key = tuple(t.data_ptr() for t in flat)
+        cached = self.__dict__.get("_weights_dev")
+        if cached is None or cached[0] != key:   # the pointer struct is rebuilt only when a parameter's storage moved
+            dev = self.device.index if self.device.index is not None else torch.cuda.current_device()
+            if any(not t.is_cuda or t.get_device() != dev or t.dtype != torch.float32 or not t.is_contiguous() for t in flat):
+                return False
+            cached = self._weights_dev = (key,) + _fill(_lib.EncoderWeights, _lib.LayerWeights, groups, _dev_ptr)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.ance_encoder_update_weights(self.h, C.byref(cached[1]), _lib.current_stream()))
+        self.__dict__.pop("_allpad", None)   # values cached per weights
+        return True
+
+    def forward_train(self, ids: torch.Tensor, lens: Optional[torch.Tensor], mask: Optional[torch.Tensor]):
+        """forward() of a whole [B, L <= 128] batch that also keeps what the backward needs.  -> (out fp32 [B, H],
+        workspace tensor for backward())."""
+        B, L = ids.shape
+        n = C.c_size_t()
+        _lib.check(self.lib.ance_encoder_train_workspace(self.h, B, L, C.byref(n)))
+        ws = torch.empty(n.value, dtype=torch.uint8, device=ids.device)
+        out = torch.empty((B, self.hidden_size), dtype=torch.float32, device=ids.device)
+        with torch.cuda.device(ids.device):
+            _lib.check(self.lib.ance_encoder_forward_train(
+                self.h, ids.data_ptr(), None if lens is None else lens.data_ptr(),
+                None if mask is None else mask.data_ptr(), B, L, ws.data_ptr(), out.data_ptr(), _lib.current_stream()))
+        return out, ws
+
+    def backward(self, d_out: torch.Tensor, ws: torch.Tensor, grads) -> None:
+        """Gradients of sum(d_out * out) for the forward_train that filled `ws`, written into `grads` (fp32 tensors
+        grouped as _param_groups)."""
+        w, lw = _fill(_lib.EncoderGrads, _lib.LayerGrads, grads, _dev_ptr)
+        with torch.cuda.device(d_out.device):
+            _lib.check(self.lib.ance_encoder_backward(self.h, d_out.data_ptr(), ws.data_ptr(), C.byref(w),
+                                                      _lib.current_stream()))
+
+
+class _TrainableEncode(torch.autograd.Function):
+    """Embeddings [B, H] of a dense batch as a function of the encoder's parameters (the `params` inputs, in
+    _param_groups order), so that their .grad accumulates and DDP's hooks fire."""
+
+    @staticmethod
+    def forward(ctx, enc, n_layer, ids, lens, mask, *params):
+        out, ws = enc.forward_train(ids, lens, mask)
+        ctx.enc, ctx.ws, ctx.n_layer = enc, ws, n_layer
+        ctx.shapes = [p.shape for p in params]
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_out):
+        dev = ctx.ws.device
+        flat = [torch.empty(s, dtype=torch.float32, device=dev) for s in ctx.shapes]
+        n = ctx.n_layer
+        groups = (flat[:5], [flat[5 + 16 * i:5 + 16 * (i + 1)] for i in range(n)], flat[5 + 16 * n:])
+        ctx.enc.backward(d_out.float().contiguous(), ctx.ws, groups)
+        return (None, None, None, None, None, *flat)
+
 
 def _forward_varlen(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
                     out: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
@@ -236,6 +325,39 @@ class _B200Encoder(nn.Module):
     #: Same tensor-core rate either way.
     encoder_operand = os.environ.get("ANCE_B200_ENCODER_OPERAND", "fp16")
 
+    #: set_trainable(True): embeddings computed while grad is enabled carry an autograd graph (dense, L <= 128)
+    _trainable = False
+
+    def set_trainable(self, on: bool = True):
+        """Opt in to gradients: while torch grad mode is on, query_emb / body_emb / encode_lens (dense batches of up to
+        128 tokens) and the triplet forward() return tensors whose backward runs the encoder's backward kernels; the
+        other encode paths raise instead of returning detached results.  Off by default."""
+        self._trainable = bool(on)
+        return self
+
+    def _grad_path(self) -> bool:
+        return self._trainable and torch.is_grad_enabled()
+
+    def _refuse_grad(self, what: str) -> None:
+        if self._grad_path():
+            raise _lib.AnceError(f"{what} has no backward: trainable encoders take dense batches of up to 128 tokens "
+                                 "through query_emb / body_emb / encode_lens (or run this under torch.no_grad())")
+
+    def _train_emb(self, enc, backbone, head, ids, lens, mask):
+        B, L = ids.shape
+        if L > 128:
+            raise _lib.AnceError(f"inputs of {L} tokens have no backward: the trainable encoder covers up to 128 tokens "
+                                 "(run longer inputs under torch.no_grad())")
+        if B * L > enc.max_tokens:
+            raise _lib.AnceError(f"a trainable batch of {B} x {L} tokens exceeds max_tokens {enc.max_tokens}")
+        # The device weights are refreshed from the parameters before every training forward, whatever their `_version`
+        # says: optimizers that write through `p.data` (the reference trainer's Lamb, transformers' AdamW) do not bump it.
+        if not enc.update_weights(backbone, head):
+            raise _lib.AnceError("a trainable encoder needs contiguous fp32 parameters on the inputs' device")
+        embs, layers, hd = _param_groups(backbone, head)
+        params = embs + [t for l in layers for t in l] + hd
+        return _TrainableEncode.apply(enc, len(layers), ids, lens, mask, *params)
+
     def _enc_for(self, name, backbone, arch, heads, pad_id, head, device) -> _CudaEncoder:
         if device.type != "cuda":
             raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback): move the model and "
@@ -249,7 +371,9 @@ class _B200Encoder(nn.Module):
             params = cache["_params"] = list(self.parameters())
         ver = (sum(p._version for p in params), params[0].data_ptr(), str(device), self.encoder_operand)
         hit = cache.get(name)
-        if hit is None or hit[0] != ver:
+        if hit is not None and hit[0] != ver and hit[0][1:] == ver[1:] and hit[1].update_weights(backbone, head):
+            cache[name] = (ver, hit[1])   # only values changed (optimizer step, load_state_dict): refreshed in place
+        elif hit is None or hit[0] != ver:
             cache[name] = (ver, _CudaEncoder(backbone, arch, heads, pad_id, head, self.max_tokens, device,
                                              self.encoder_operand))
         return cache[name][1]
@@ -270,18 +394,23 @@ class _B200Encoder(nn.Module):
         mask = (attention_mask != 0).to(torch.uint8).contiguous()
         return ids, mask
 
-    # -- reference `NLL.forward` (model/models.py:58-84), EVALUATION ONLY ---------------------------------------
+    # -- reference `NLL.forward` (model/models.py:58-84) ------------------------------------------------------
     # Same signature and return values as the reference: embeddings when only one side is given, `(loss,)` for a
-    # (query, positive, negative) triplet batch.  The encoder kernels have no backward pass, so the loss carries no
-    # autograd graph (training stays with the reference trainer, SURVEY.md par. 8(f) row 3); it is what the trainer
-    # logs, computed with the refresher's weights.
+    # (query, positive, negative) triplet batch.  After set_trainable(True), with grad enabled, the loss carries an
+    # autograd graph through the encoder's backward kernels (inputs of up to 128 tokens); otherwise it is computed
+    # under no_grad, as the value the trainer logs.
     @staticmethod
     def _pair_logits(q_embs, x_embs, input_ids_x, attention_mask_x):
         return (q_embs * x_embs).sum(-1)
 
-    @torch.no_grad()
     def forward(self, query_ids, attention_mask_q, input_ids_a=None, attention_mask_a=None, input_ids_b=None,
                 attention_mask_b=None, is_query=True):
+        with contextlib.nullcontext() if self._grad_path() else torch.no_grad():
+            return self._nll_forward(query_ids, attention_mask_q, input_ids_a, attention_mask_a, input_ids_b,
+                                     attention_mask_b, is_query)
+
+    def _nll_forward(self, query_ids, attention_mask_q, input_ids_a, attention_mask_a, input_ids_b, attention_mask_b,
+                     is_query):
         if input_ids_b is None and is_query:
             return self.query_emb(query_ids, attention_mask_q)
         if input_ids_b is None:
@@ -355,6 +484,9 @@ class RobertaDot_NLL_LN(_B200Encoder):
 
     def query_emb(self, input_ids, attention_mask):
         ids, mask = self._prep(input_ids, attention_mask)
+        if self._grad_path():
+            return self._train_emb(self._encoder(ids.device), self.roberta, (self.embeddingHead, self.norm), ids, None,
+                                   mask)
         return self._encoder(ids.device).forward(ids, None, mask)
 
     def body_emb(self, input_ids, attention_mask):
@@ -362,6 +494,10 @@ class RobertaDot_NLL_LN(_B200Encoder):
 
     # fast path used by the GPU refresher: mask given as lengths (msmarco_data.py:282 form)
     def encode_lens(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if self._grad_path() and out is None:
+            return self._train_emb(self._encoder(ids_i32.device), self.roberta, (self.embeddingHead, self.norm),
+                                   ids_i32.contiguous(), lens_i32.contiguous(), None)
+        self._refuse_grad("encode_lens(out=...)")
         return self._encoder(ids_i32.device).forward(ids_i32.contiguous(), lens_i32.contiguous(), None, out=out)
 
     def encode_lens_varlen(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
@@ -370,6 +506,7 @@ class RobertaDot_NLL_LN(_B200Encoder):
         attention tiles.  align = 1: densest packing, embeddings equal encode_lens up to fp32 summation order inside a
         tile; align = 16: bit-identical to encode_lens and independent of the batch composition (~12 % fewer real tokens
         per tile).  L <= 128 (the MS MARCO passage and query caches); longer caches use encode_lens_bucketed."""
+        self._refuse_grad("encode_lens_varlen")
         return self._encoder(ids_i32.device).forward_varlen(ids_i32.contiguous(), lens_i32.contiguous(), lens_host, out=out,
                                                             align=align)
 
@@ -378,6 +515,7 @@ class RobertaDot_NLL_LN(_B200Encoder):
         """encode_lens at the cost of the REAL tokens only, for any L <= 512 (lengths in [1, L]).  align = 16: bit-identical
         to encode_lens at the same L, whatever else is in the batch; align = 1: densest packing, equal up to fp32
         summation order.  L <= 128 is encode_lens_varlen."""
+        self._refuse_grad("encode_lens_packed")
         return self._encoder(ids_i32.device).forward_packed(ids_i32.contiguous(), lens_i32.contiguous(), lens_host, out=out,
                                                             align=align)
 
@@ -387,6 +525,7 @@ class RobertaDot_NLL_LN(_B200Encoder):
         smallest supported padded length >= their own length (16/32/64/128/256/384/512) and each group is
         encoded at that length.  Padding keys carry the additive -10000 (probability exactly 0 in fp32) and
         padding rows are never read, so dropping trailing pad columns does not change a sequence's embedding."""
+        self._refuse_grad("encode_lens_bucketed")
         B, L = ids_i32.shape
         buckets = [b for b in (8, 16, 32, 64) if min_bucket <= b < L] + [b for b in range(128, L + 1, 128)]
         if not buckets or buckets[-1] != L:
@@ -411,6 +550,7 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
         self.base_len = 512
 
     def body_emb(self, input_ids, attention_mask):
+        self._refuse_grad("the multi-chunk body_emb")
         batchS, full_length = input_ids.shape
         chunk_factor = full_length // self.base_len
         if chunk_factor == 0 or full_length % chunk_factor != 0:
@@ -432,6 +572,7 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
 
     def encode_lens_multi_chunk(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor) -> torch.Tensor:
         """[B, full] ids + document lengths -> [B, chunks, 768]; chunk c sees max(0, min(512, len - 512c)) tokens."""
+        self._refuse_grad("encode_lens_multi_chunk")
         B, full = ids_i32.shape
         cf = full // self.base_len
         seq = full // cf
@@ -446,6 +587,7 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
         the packed forward (align as in encode_lens_packed; 16 = bit-identical); an all-padding chunk (length 0, every id
         pad_id, as the token caches store them) gets the one vector such a chunk has, computed once per encoder and
         weights by the dense forward; any other empty chunk is encoded densely."""
+        self._refuse_grad("encode_lens_multi_chunk_packed")
         B, full = ids_i32.shape
         cf = full // self.base_len
         seq = full // cf
@@ -511,6 +653,11 @@ class BiEncoder(_B200Encoder):
                                         d.max_position_embeddings, d.type_vocab_size, d.pad_token_id, d.layer_norm_eps)
         self.ctx_model = _backbone(d.vocab_size, d.hidden_size, d.num_hidden_layers, d.intermediate_size,
                                    d.max_position_embeddings, d.type_vocab_size, d.pad_token_id, d.layer_norm_eps)
+
+    def set_trainable(self, on: bool = True):
+        if on:
+            raise NotImplementedError("the DPR BiEncoder has no backward in ance_b200 (rdot_nll only)")
+        return super().set_trainable(False)
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         # HF BertModel checkpoints carry pooler.* and position_ids buffers the path never uses

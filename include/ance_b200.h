@@ -14,6 +14,7 @@
 #ifndef ANCE_B200_H_
 #define ANCE_B200_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -223,6 +224,46 @@ int ance_encoder_check(ance_encoder_t enc, void* stream);
 int ance_encoder_debug_hidden(ance_encoder_t enc, int layer, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training: gradients of the dense forward for sequences of up to 128 tokens (the trainer side of
+ * model/models.py:58-84, NLL.forward -> loss.backward()).
+ * ------------------------------------------------------------------------------------------------ */
+/* Gradient buffers: the layout of ance_encoder_weights / ance_layer_weights with DEVICE fp32 pointers (16-byte aligned),
+ * every one required (the head's only with has_head).  ance_encoder_backward OVERWRITES them. */
+typedef struct {
+  float *q_w, *q_b, *k_w, *k_b, *v_w, *v_b;
+  float *ao_w, *ao_b, *ln1_g, *ln1_b;
+  float *ff1_w, *ff1_b;
+  float *ff2_w, *ff2_b, *ln2_g, *ln2_b;
+} ance_layer_grads;
+
+typedef struct {
+  float *word_emb, *pos_emb, *type_emb, *emb_ln_g, *emb_ln_b;
+  const ance_layer_grads* layers;                    /* [n_layer], host array of device pointers */
+  float *head_w, *head_b, *head_ln_g, *head_ln_b;
+} ance_encoder_grads;
+
+/* Bytes of device workspace one ance_encoder_forward_train of a [B, L] batch keeps for its backward (about
+ * 16 hidden + 4 ffn bytes per token and layer: 24.6 KB at hidden 768, ffn 3072).  ANCE_ERR_UNSUPPORTED for L > 128. */
+int ance_encoder_train_workspace(ance_encoder_t enc, int B, int L, size_t* bytes);
+/* ance_encoder_forward with every activation the backward needs saved in ws_dev (256-byte aligned, the size above; one
+ * workspace per forward whose backward is still to come; each forward_train is followed by at most one backward).  out_dev is bit-identical to ance_encoder_forward's.
+ * L must be 8, 16, 32, 64 or 128 (ANCE_ERR_UNSUPPORTED above 128) and B * L <= max_tokens. */
+int ance_encoder_forward_train(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev,
+                               int B, int L, void* ws_dev, float* out_dev, void* stream);
+/* Gradients of sum(d_out o out) with respect to every weight, for the forward that filled ws_dev (the weights must not
+ * have changed since).  d_out_dev [B, hidden] fp32, 16-byte aligned.  The handle forgets ws_dev once this call is made:
+ * a second backward from the same workspace is ANCE_ERR_INVALID.  Backward GEMM operands are bf16 whatever operand_fmt is, with fp32
+ * accumulation; residual-stream and weight gradients are fp32.  Weight rows that the reference declares as padding_idx get
+ * no gradient (word row pad_id; position row pad_id for RoBERTa).  The word / position gradients are scatter-added with
+ * fp32 atomics: their summation order, and so their last bits, vary from run to run; everything else is deterministic. */
+int ance_encoder_backward(ance_encoder_t enc, const float* d_out_dev, void* ws_dev, const ance_encoder_grads* g,
+                          void* stream);
+/* In-place weight refresh (after an optimizer step): w_dev holds DEVICE fp32 pointers in the layout of ance_encoder_create's
+ * weights; they are converted into the handle's existing buffers in stream order, without a host round trip or a new
+ * allocation.  The result is the handle ance_encoder_create would build from the same values. */
+int ance_encoder_update_weights(ance_encoder_t enc, const ance_encoder_weights* w_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Device-time profile by kernel class (bench.py's roofline numbers): CUDA events recorded around every
  * launch on the launch stream.  Classes: 0 encoder GEMM, 1 attention, 2 LayerNorm/embedding/gather,
  * 3 operand quantisation, 4 coarse search GEMM, 5 exact rescore, 6 exact brute force, 7-10 encoder
@@ -275,6 +316,28 @@ int ance_dbg_attention(int fmt, const void* qkv_dev, int n_tokens, int L, int he
 int ance_dbg_layer_norm(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H, const float* gamma_dev,
                         const float* beta_dev, float eps, void* out16_dev, float* out32_dev, int rows_per_warp,
                         void* stream);
+/* The backward's attention kernel: qkv [B * L, 3 * 64 heads] 16-bit in `fmt` and kbias [B * L] as for ance_dbg_attention
+ * (dense, L <= 128), dout [B * L, 64 heads] bf16 (cls_only: [B, 64 heads], the gradient of token 0 of each sequence only)
+ * -> dqkv [B * L, 3 * 64 heads] fp32. */
+int ance_dbg_attention_backward(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                int cls_only, int B, int L, int heads, float* dqkv_dev, void* stream);
+/* The backward's LayerNorm kernel: input rows as for ance_dbg_layer_norm, dy / dx fp32 [rows, H]; dgamma, dbeta and dsum
+ * (column sum of dx) [H] may each be null. */
+int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
+                                 const float* gamma_dev, float eps, const float* dy_dev, float* dx_dev, float* dgamma_dev,
+                                 float* dbeta_dev, float* dsum_dev, void* stream);
+/* The backward's GELU kernel: g[i] *= gelu'(u[i]) for n elements, u 16-bit in `fmt`, g fp32. */
+int ance_dbg_gelu_backward(int fmt, const void* u_dev, float* g_dev, int64_t n, void* stream);
+/* The backward's embedding kernels: E [B * L, H] fp32 = (word[id] + pos[p]) + type[0], the LayerNorm input the backward
+ * recomputes (positions by the arch's rule, roberta = 1 for RoBERTa's), then dword [vocab, H] and dpos [max_pos, H] are
+ * zeroed and the rows of dE [B * L, H] scatter-added into them (no gradient for the padding_idx rows).  L <= 128. */
+int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int roberta, int pad_id, int vocab, int max_pos,
+                                const float* word_dev, const float* pos_dev, const float* type_dev, const float* dE_dev,
+                                float* E_dev, float* dword_dev, float* dpos_dev, void* stream);
+/* The backward's transpose: dst [C, dst_ld] bf16 = src [R, C]^T (src rows at pitch src_ld; src_kind 0 fp16, 1 bf16, 2 fp32),
+ * columns R .. dst_ld - 1 of dst set to zero. */
+int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, int R, int C, void* dst_dev, int64_t dst_ld,
+                            void* stream);
 
 #ifdef __cplusplus
 }
