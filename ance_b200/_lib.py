@@ -108,6 +108,7 @@ SIGNATURES = {
                                              C.c_void_p, C.c_void_p, C.c_void_p]),
     "ance_encoder_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(EncoderGrads), C.c_void_p]),
     "ance_encoder_update_weights": (C.c_int, [C.c_void_p, C.POINTER(EncoderWeights), C.c_void_p]),
+    "ance_encoder_debug_grads": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ance_profile_enable": (C.c_int, [C.c_int]),
     "ance_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "ance_dbg_pack_varlen": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -131,7 +132,12 @@ SIGNATURES = {
     "ance_dbg_embedding_backward": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p] * 8),
     "ance_dbg_transpose_bf16": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p]),
+    "ance_dbg_train_layout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
 }
+
+# ance_dbg_train_layout's fields, in order
+TRAIN_LAYOUT_FIELDS = ("ids", "kbias", "layers", "per_layer", "x_in", "qkv", "ctx", "t1", "x1", "u", "ff", "t2",
+                       "x_final", "head_in", "total")
 
 
 def lib_path() -> Path:

@@ -433,6 +433,9 @@ struct ance_encoder {
   int* err_flag = nullptr;
   uint16_t* dbg = nullptr;       // [(n_layer+1), max_tokens, H] when debugging
   int dbg_tokens = 0;
+  float* dbg_grads = nullptr;    // [(n_layer+1), dbg_grads_tokens, H]: backward residual-stream gradients (debug_grads)
+  int dbg_grads_tokens = 0;
+  bool dbg_grads_valid = false;  // the last backward was captured (a larger one leaves the slots unwritten)
   int prune_last_layer = 1;  // last layer: only the CLS rows go through out-proj / FFN (identical result)
   int varlen_align = 1;      // ance_encoder_forward_varlen / _packed: 1 = densest, 16 = exact packing, see pack_chunk
   std::vector<void*> allocs;
@@ -635,6 +638,8 @@ int run_attention(const AttentionLaunch& a, cudaStream_t st) {
 struct TrainLayout {
   size_t ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total;
 };
+constexpr int kTrainLayoutFields = 15;   // ance_dbg_train_layout returns them in this order
+static_assert(sizeof(TrainLayout) == kTrainLayoutFields * sizeof(size_t), "ance_dbg_train_layout lists every field");
 
 TrainLayout train_layout(const ance_encoder_config& c, int B, int L) {
   const size_t M = static_cast<size_t>(B) * L, H = c.hidden, F = c.ffn;
@@ -1075,6 +1080,13 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
   } else {
     ANCE_CUDA(cudaMemcpyAsync(s.G, d_out, static_cast<size_t>(B) * H * 4, cudaMemcpyDeviceToDevice, st));
   }
+  const bool capture = e->dbg_grads && M <= e->dbg_grads_tokens;   // ance_encoder_debug_grads: slot l = d X_in(l)
+  e->dbg_grads_valid = capture;
+  auto capture_g = [&](int slot, int rows) {
+    return cudaMemcpyAsync(e->dbg_grads + static_cast<size_t>(slot) * e->dbg_grads_tokens * H, s.G,
+                           static_cast<size_t>(rows) * H * 4, cudaMemcpyDeviceToDevice, st);
+  };
+  if (capture) ANCE_CUDA(capture_g(NL, B));
   for (int l = NL - 1; l >= 0; --l) {
     const LayerDev& d = e->layers[l];
     const ance_encoder::LayerT& wt = e->wt[l];
@@ -1119,6 +1131,7 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
       if ((rc = wgrad(s.Gt + static_cast<size_t>(p) * H * Mp, H, s.Xt, H, Mp, wq[p], st))) return rc;
     if ((rc = linear<kBF>(s.A16, 3 * H, M, wt.wqkv, H, 3 * H, nullptr, nullptr, 0, nullptr, s.G, st))) return rc;   // d X_in
     if ((rc = add_rows(s.G, last ? L : 1, s.dT, Mr, H, st))) return rc;   // + residual (the CLS rows in the last layer)
+    if (capture) ANCE_CUDA(capture_g(l, M));
   }
   // embeddings: X0 = LN((word[id] + pos[p]) + type[0])
   {
@@ -1555,6 +1568,37 @@ extern "C" int ance_encoder_debug_hidden(ance_encoder_t e, int layer, float* out
   if (e->fmt == tc05::kFmtBF16) act16_to_f32_kernel<tc05::kFmtBF16><<<blocks, 256, 0, st>>>(e->dbg + static_cast<size_t>(layer) * n, out_dev, n);
   else act16_to_f32_kernel<tc05::kFmtF16><<<blocks, 256, 0, st>>>(e->dbg + static_cast<size_t>(layer) * n, out_dev, n);
   ANCE_CUDA(cudaGetLastError());
+  return ANCE_OK;
+}
+
+extern "C" int ance_encoder_debug_grads(ance_encoder_t e, int slot, float* out_dev, void* stream) {
+  ANCE_REQUIRE(e != nullptr, "ance_encoder_debug_grads: null handle");
+  const size_t H = e->cfg.hidden;
+  if (slot < 0) {  // enable capture for backwards of up to 4096 tokens
+    if (!e->dbg_grads) {
+      e->dbg_grads_tokens = std::min(e->max_tokens, 4096);
+      e->dbg_grads = dev_alloc<float>(e, static_cast<size_t>(e->cfg.n_layer + 1) * e->dbg_grads_tokens * H);
+      ANCE_REQUIRE(e->dbg_grads != nullptr, "ance_encoder_debug_grads: allocation failed");
+    }
+    return ANCE_OK;
+  }
+  ANCE_REQUIRE(e->dbg_grads != nullptr, "ance_encoder_debug_grads: capture not enabled (call with slot = -1 first)");
+  ANCE_REQUIRE(e->dbg_grads_valid, "ance_encoder_debug_grads: the last backward was not captured (none since capture was "
+               "enabled, or more than %d tokens)", e->dbg_grads_tokens);
+  ANCE_REQUIRE(slot <= e->cfg.n_layer && out_dev, "ance_encoder_debug_grads: bad slot %d or null buffer", slot);
+  const size_t n = static_cast<size_t>(e->dbg_grads_tokens) * H;
+  ANCE_CUDA(cudaMemcpyAsync(out_dev, e->dbg_grads + static_cast<size_t>(slot) * n, n * 4, cudaMemcpyDeviceToDevice,
+                            reinterpret_cast<cudaStream_t>(stream)));
+  return ANCE_OK;
+}
+
+extern "C" int ance_dbg_train_layout(ance_encoder_t e, int B, int L, size_t* out) {
+  ANCE_REQUIRE(e != nullptr && out != nullptr, "ance_dbg_train_layout: null argument");
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= attn::kTile, "ance_dbg_train_layout: need B > 0 and 0 < L <= 128 (B = %d, L = %d)", B, L);
+  const TrainLayout t = train_layout(e->cfg, B, L);
+  const size_t f[kTrainLayoutFields] = {t.ids, t.kbias, t.layers, t.per_layer, t.x_in, t.qkv, t.ctx, t.t1,
+                                        t.x1, t.u, t.ff, t.t2, t.x_final, t.head_in, t.total};
+  memcpy(out, f, sizeof(f));
   return ANCE_OK;
 }
 

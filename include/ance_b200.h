@@ -262,6 +262,14 @@ int ance_encoder_backward(ance_encoder_t enc, const float* d_out_dev, void* ws_d
  * weights; they are converted into the handle's existing buffers in stream order, without a host round trip or a new
  * allocation.  The result is the handle ance_encoder_create would build from the same values. */
 int ance_encoder_update_weights(ance_encoder_t enc, const ance_encoder_weights* w_dev, void* stream);
+/* Debug / tests: the residual-stream gradients of the last ance_encoder_backward.  slot = -1 enables capture for backwards
+ * of up to min(max_tokens, 4096) tokens (allocates (n_layer + 1) x that x hidden fp32; off by default).  With capture on,
+ * slot n_layer holds d x_final [B, hidden] (the gradient into the last layer's CLS outputs, after the head; d_out itself
+ * without a head) and slot l < n_layer holds d X_in(l) [B * L, hidden], the gradient into layer l's input (slot 0: into the
+ * embedding LayerNorm's output).  slot >= 0 copies a whole slot, [min(max_tokens, 4096), hidden] fp32, into out_dev; it
+ * is ANCE_ERR_INVALID when the last backward was not captured (none since capture was enabled, or one of more tokens than
+ * the limit), so a read never returns an earlier backward's gradients. */
+int ance_encoder_debug_grads(ance_encoder_t enc, int slot, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Device-time profile by kernel class (bench.py's roofline numbers): CUDA events recorded around every
@@ -338,6 +346,14 @@ int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int
  * columns R .. dst_ld - 1 of dst set to zero. */
 int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, int R, int C, void* dst_dev, int64_t dst_ld,
                             void* stream);
+/* Host-only: the byte offsets of the workspace ance_encoder_forward_train fills for a [B, L <= 128] batch, out[15] =
+ * ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total.  ids [B * L] int32 and kbias
+ * [B * L] fp32 (log2 units) sit at their offsets; layer l's slots at layers + l * per_layer + (x_in .. t2); x_final
+ * [B, hidden] 16-bit (the last layer's CLS outputs) and head_in [B, hidden] fp32 (the head LayerNorm's input) at theirs.
+ * Every slot has room for B * L rows and is 16-bit in operand_fmt: x_in, ctx, t1, x1, t2 [., hidden], qkv [., 3 hidden],
+ * u, ff [., ffn].  In the pruned last layer T1, X1, U, FF and T2 are compact: row b is sequence b's CLS row (B rows used);
+ * CTX keeps its B * L rows (the CLS rows are read at pitch L * hidden); X_in and QKV are full. */
+int ance_dbg_train_layout(ance_encoder_t enc, int B, int L, size_t* out);
 
 #ifdef __cplusplus
 }

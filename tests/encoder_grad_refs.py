@@ -84,7 +84,9 @@ def attention_bwd_tol(qkv, kbias_log2, dout, B, L, heads):
     # the score is formed in fp32 in log2 units beside the -10000 log2(e) key bias: its rounding, u |s|, is the larger term
     # on masked keys (all-padding rows)
     ds_err = _g(64) * (q @ k.transpose(-1, -2)) / 8.0 + 2 * U32 * s_log2.abs() / math.log2(math.e)
-    eps_p = 2.0 * ds_err.amax(-1, keepdim=True) + 8 * U32
+    # a masked key of a row that has an unmasked one sits ~14427 log2 units below the row maximum: exp2f of it is 0 in
+    # the kernel and P = 0 here, whatever the score's rounding, so only keys with P > 0 set the row's eps_P
+    eps_p = 2.0 * (ds_err * (p > 0)).amax(-1, keepdim=True) + 8 * U32
     adp = do @ v.transpose(-1, -2)
     pd = (p * adp).sum(-1, keepdim=True)
     ads = p * (adp + pd)                                          # |dS| with no cancellation
