@@ -7,21 +7,25 @@
 // (bias added in fp32 before the softmax), so an all-padding sequence gives the same finite
 // "softmax of the raw scores" the reference gives, not NaN.
 //
-// One work item = (128-token query tile, head); a persistent CTA per SM walks its items while a TMA producer warp
-// streams Q / K / V up to kStages key blocks ahead.  Per 128-key block of the same sequence:
+// Two kernels, both over work items (128-token query tile, head) and persistent (one CTA per SM):
+//   attention_single_kernel   one 128-key block per item (L <= 128 dense or packed, row plans of sequences of up to 128
+//                             tokens): warp-specialised, two MMA warpgroups with S, P and O in registers (below)
+//   attention_multi_kernel    several key blocks per item (L = 256 / 512, packed sequences longer than 128): a TMA
+//                             producer warp streams Q / K / V up to kStages key blocks ahead of one warpgroup that runs,
+//                             per 128-key block of the same sequence:
 //   S = Q K^T          wgmma m64n128k16 x (2 x 4)   (Q, K: TMA boxes of the [tokens, 3H] QKV buffer), written to a
 //                      shared fp32 score tile
-//   softmax            one warpgroup, thread = query row reading its row of the score tile: L <= 128 one pass (row in
-//                      registers: max, exp2), L > 128 two passes per block with online rescaling;
-//                      P written as 16-bit (FMT) into shared memory in the K-major SWIZZLE_128B layout
+//   softmax            one warpgroup, thread = query row reading its row of the score tile, two passes per block with
+//                      online rescaling; P written as 16-bit (FMT) into shared memory in the K-major SWIZZLE_128B layout
 //   O_blk = P V        wgmma m64n64k16 x (2 x 8)    (V is the MN-major B operand), written over the score tile
 //   o = o*alpha + O_blk in registers; after the last block ctx = o / l  (16-bit)
 // Sequence lengths: a multiple of 128, or a divisor of 128 (then a tile holds 128/L sequences and
 // cross-sequence scores are excluded).  head_dim is fixed at 64 (BERT/RoBERTa-base).
 // Packed variable-length token matrices (kPacked with a row plan): every row r attends to the keys [row_lo[r], row_hi[r])
-// of its own sequence.  kSingle: no sequence straddles a 128-row tile.  Otherwise an item's keys are the contiguous packed
-// rows [kv0, kv0 + 128 nkv) covering every row's own range (tile_kv); the blocks of it outside a row's range are exact
-// no-ops for that row, and the first block inside it takes the two-pass treatment the dense kernel gives block 0.
+// of its own sequence.  Single-block plans: no sequence straddles a 128-row tile.  Otherwise an item's keys are the
+// contiguous packed rows [kv0, kv0 + 128 nkv) covering every row's own range (tile_kv); the blocks of it outside a row's
+// range are exact no-ops for that row, and the first block inside it takes the two-pass treatment the dense kernel gives
+// block 0.
 #pragma once
 #include "act16.cuh"
 #include "tc05.cuh"
@@ -51,7 +55,7 @@ struct Params {
   // zero), rows that belong to no sequence attend to themselves only.
   const int32_t* row_lo;
   const int32_t* row_hi;
-  // kPacked && !kSingle: per 128-row tile, (first key row, number of 128-key blocks) of its work items
+  // attention_multi_kernel<kPacked = true>: per 128-row tile, (first key row, number of 128-key blocks) of its work items
   const int2* tile_kv;
 };
 
@@ -76,17 +80,16 @@ struct Smem {
 // a running maximum above this is the score of an unmasked key: masked keys sit near -10000 log2(e) = -14427
 constexpr float kRealMax = -7000.0f;
 
-constexpr int kThreads = 256;   // warp 0 TMA, 1-3 idle, 4-7 the softmax / MMA warpgroup
+constexpr int kThreads = 256;   // attention_multi_kernel: warp 0 TMA, 1-3 idle, 4-7 the softmax / MMA warpgroup
 
 // Persistent, one CTA per SM.  The CTA walks its work items w = blockIdx.x + n * gridDim.x; the TMA producer runs
 // up to kStages key/value blocks ahead (the HBM latency of a 48 KB Q/K/V fetch is longer than one item's
 // arithmetic); producer and warpgroup derive the block order from the same loop nest.
-// kPacked: L < 128, a tile holds 128/L sequences; or a variable-length row plan (p.row_lo).  kSingle: one key block per
-// item (L <= 128, or a plan whose sequences never straddle a tile).
+// kPacked: a variable-length row plan (p.row_lo, p.tile_kv) of sequences longer than 128 tokens.
 // FMT: 16-bit format of Q / K / V, of the probabilities P and of the output (act16.cuh).
-template <bool kPacked, bool kSingle, uint32_t FMT>
+template <bool kPacked, uint32_t FMT>
 __global__ void __launch_bounds__(kThreads, 1)
-attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
+attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Smem::kBar);
@@ -101,7 +104,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
   const int nkv_dense = (p.L >= kTile) ? p.L / kTile : 1;
   // keys of the items of a tile: first key row, number of 128-key blocks
   auto kv_of = [&](int tile, int& kv0, int& nkv) {
-    if constexpr (kPacked && !kSingle) {
+    if constexpr (kPacked) {
       const int2 t = __ldg(p.tile_kv + tile);
       kv0 = t.x;
       nkv = t.y;
@@ -199,10 +202,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
       const int seq_full = seq_lo + ((seq_hi - seq_lo) & ~31);
       float m_run = -INFINITY, l_run = 0.f;
       float o[kDh];
-      if constexpr (!kSingle) {
 #pragma unroll
-        for (int i = 0; i < kDh; ++i) o[i] = 0.f;
-      }
+      for (int i = 0; i < kDh; ++i) o[i] = 0.f;
       for (int j = 0; j < nkv; ++j) {
         // key bias of this block -> smem (the previous block's readers are past their last use: they all passed
         // the barrier after the P V of that block)
@@ -229,7 +230,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
           // the unmasked chunks of the dense kernel do; the others take the dense kernel's partial-chunk arithmetic)
 #pragma unroll
           for (int c = 0; c < 4; ++c)
-            st[c] = (bh <= c * 32 || bl >= c * 32 + 32) ? 0 : (bl <= c * 32 && (kSingle ? bh : bf) >= c * 32 + 32) ? 1 : 2;
+            st[c] = (bh <= c * 32 || bl >= c * 32 + 32) ? 0 : (bl <= c * 32 && bf >= c * 32 + 32) ? 1 : 2;
         } else {
           bool own[4], any_unmasked = false;
 #pragma unroll
@@ -237,7 +238,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
             own[c] = !kPacked || (p.L >= 32 ? (c * 32 >= seq_lo && c * 32 < seq_hi) : c == quad);
             any_unmasked |= own[c] && mk[c] != 0xffffffffu;
           }
-          const bool skip_ok = (kPacked && p.L < 32) ? false : (any_unmasked || (!kSingle && m_run > kRealMax));
+          const bool skip_ok = (kPacked && p.L < 32) ? false : (any_unmasked || m_run > kRealMax);
 #pragma unroll
           for (int c = 0; c < 4; ++c)
             st[c] = !own[c] ? 0 : (mk[c] == 0xffffffffu && skip_ok) ? 0 : (mk[c] == 0u && !(kPacked && p.L < 32)) ? 1 : 2;
@@ -271,164 +272,108 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
         }
         named_bar_sync(bar_id, kTile);   // every row of S is in the tile
         float rsum, alpha = 1.f, m_new;
-        bool all_skip = false;
-        if constexpr (kSingle) {
-          // one key block per item: the whole score row lives in registers, one read of the score tile
-          uint32_t v[kTile];
-#pragma unroll
-          for (int c = 0; c < kTile; c += 32) acc_ld_x32(srow + c, v + c);
-          float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-          if (plain) {   // max of the raw scores: scale > 0 commutes with max
-#pragma unroll
-            for (int i = 0; i < kTile; ++i) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(v[i]));
-          } else {
-#pragma unroll
-            for (int c = 0; c < kTile; c += 32) {
-              if (st[c >> 5] == 1) {
-#pragma unroll
-                for (int i = c; i < c + 32; ++i) {
-                  const float t = __uint_as_float(v[i]) * p.scale_log2;
-                  v[i] = __float_as_uint(t);
-                  mx[i & 3] = fmaxf(mx[i & 3], t);
-                }
-              } else if (st[c >> 5] == 2) {
-#pragma unroll
-                for (int i = c; i < c + 32; ++i) {
-                  float t = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[i]);
-                  if (kPacked && (i < bl || i >= bh)) t = -INFINITY;
-                  v[i] = __float_as_uint(t);
-                  mx[i & 3] = fmaxf(mx[i & 3], t);
-                }
-              }
-            }
-          }
-          m_new = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-          const float sc = plain ? p.scale_log2 : 1.0f;
-          if (plain) m_new *= p.scale_log2;
-          const float nm = -m_new;
-          float rs[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
+        const int stb = st[0] | (st[1] << 2) | (st[2] << 4) | (st[3] << 6);
+        const bool all_skip = stb == 0;   // a fully masked block of a row that has real keys: contributes nothing
+        // p = exp2(t - m_ref) for the whole block: row sum, 16-bit P into swizzled smem; returns max(t - m_ref)
+        auto exp_pass = [&](float m_ref, float& rs_out) -> float {
+          float rs_ = 0.f, mu = -INFINITY;
+          const float nm = -m_ref;
+#pragma unroll 1
           for (int c = 0; c < kTile; c += 32) {
+            const int sc_ = (stb >> (c >> 4)) & 3;
             uint32_t pk[16];
-            if (st[c >> 5] == 0) {
+            if (sc_ == 0) {
 #pragma unroll
               for (int i = 0; i < 16; ++i) pk[i] = 0u;
             } else {
+              uint32_t v[32];
+              acc_ld_x32(srow + c, v);
+              if (sc_ == 1) {
 #pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float p0 = ex2_ftz(fmaf(__uint_as_float(v[c + i]), sc, nm));
-                const float p1 = ex2_ftz(fmaf(__uint_as_float(v[c + i + 1]), sc, nm));
-                rs[(i >> 1) & 3] += p0 + p1;
-                pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
+                for (int i = 0; i < 32; i += 2) {
+                  const float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, nm);
+                  const float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, nm);
+                  mu = fmaxf(mu, fmaxf(u0, u1));
+                  const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
+                  rs_ += p0 + p1;
+                  pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
+                }
+              } else {
+#pragma unroll
+                for (int i = 0; i < 32; i += 2) {
+                  float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]) + nm;
+                  float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, sbias[c + i + 1]) + nm;
+                  if constexpr (kPacked) {   // other sequences' keys: nothing; keys of whole chunks: unmasked arithmetic
+                    const int k0 = c + i, k1 = c + i + 1;
+                    u0 = (k0 < bl || k0 >= bh) ? -INFINITY : (k0 < bf) ? fmaf(__uint_as_float(v[i]), p.scale_log2, nm) : u0;
+                    u1 = (k1 < bl || k1 >= bh) ? -INFINITY : (k1 < bf) ? fmaf(__uint_as_float(v[i + 1]), p.scale_log2, nm) : u1;
+                  }
+                  mu = fmaxf(mu, fmaxf(u0, u1));
+                  const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
+                  rs_ += p0 + p1;
+                  pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
+                }
               }
             }
             store_chunks(sP + (c >> 6) * (kTile * 128) + row * 128, (c & 63) >> 3, pk);
           }
-          rsum = (rs[0] + rs[1]) + (rs[2] + rs[3]);
+          rs_out = rs_;
+          return mu;
+        };
+        // Blocks after the first: ONE trip over the scores, relative to the running maximum (the block's own maximum is
+        // tracked on the way).  exp2(t - m_run) stays <= 2^8 unless a score exceeds every earlier one by more than 8
+        // (log2 units) — then, and only then, the warp redoes the block relative to the true maximum.  The softmax is
+        // the same function either way (numerator and denominator carry the same factor 2^(m_true - m_ref)).
+        const bool optimistic = __all_sync(0xffffffffu, j > 0 && m_run > kRealMax);
+        // (packed tiles: all_skip may differ between the rows of a warp, so the vote is taken by every lane; a skipped
+        // row has over = -inf, and a redo leaves it as it was: m_new = m_run, alpha = 1, P = 0)
+        if (optimistic) {
+          m_new = m_run;
+          alpha = 1.f;
+          rsum = 0.f;
+          float over = -INFINITY;
+          if (!all_skip) {
+            over = exp_pass(m_run, rsum);
+          } else {
+            float dummy;
+            exp_pass(m_run, dummy);   // (writes the zero P tile; no score reads: every chunk state is 0)
+          }
+          if (__any_sync(0xffffffffu, over > 8.0f)) {
+            m_new = fmaxf(m_run, m_run + over);
+            alpha = exp2f(m_run - m_new);
+            exp_pass(m_new, rsum);
+          }
         } else {
-          const int stb = st[0] | (st[1] << 2) | (st[2] << 4) | (st[3] << 6);
-          all_skip = stb == 0;   // a fully masked block of a row that has real keys: contributes nothing
-          // p = exp2(t - m_ref) for the whole block: row sum, 16-bit P into swizzled smem; returns max(t - m_ref)
-          auto exp_pass = [&](float m_ref, float& rs_out) -> float {
-            float rs_ = 0.f, mu = -INFINITY;
-            const float nm = -m_ref;
+          // first block of an item (or no real key seen yet): pass 1 = row max (of the raw scores when `plain`:
+          // scale > 0 commutes with max), pass 2 = exp relative to it
+          float m_blk = -INFINITY;
+          if (!all_skip) {
 #pragma unroll 1
             for (int c = 0; c < kTile; c += 32) {
               const int sc_ = (stb >> (c >> 4)) & 3;
-              uint32_t pk[16];
-              if (sc_ == 0) {
+              if (sc_ == 0) continue;
+              uint32_t v[32];
+              acc_ld_x32(srow + c, v);
+              if (plain) {
 #pragma unroll
-                for (int i = 0; i < 16; ++i) pk[i] = 0u;
+                for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]));
+              } else if (sc_ == 1) {
+#pragma unroll
+                for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]) * p.scale_log2);
               } else {
-                uint32_t v[32];
-                acc_ld_x32(srow + c, v);
-                if (sc_ == 1) {
 #pragma unroll
-                  for (int i = 0; i < 32; i += 2) {
-                    const float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, nm);
-                    const float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, nm);
-                    mu = fmaxf(mu, fmaxf(u0, u1));
-                    const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
-                    rs_ += p0 + p1;
-                    pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
-                  }
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 32; i += 2) {
-                    float u0 = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]) + nm;
-                    float u1 = fmaf(__uint_as_float(v[i + 1]), p.scale_log2, sbias[c + i + 1]) + nm;
-                    if constexpr (kPacked) {   // other sequences' keys: nothing; keys of whole chunks: unmasked arithmetic
-                      const int k0 = c + i, k1 = c + i + 1;
-                      u0 = (k0 < bl || k0 >= bh) ? -INFINITY : (k0 < bf) ? fmaf(__uint_as_float(v[i]), p.scale_log2, nm) : u0;
-                      u1 = (k1 < bl || k1 >= bh) ? -INFINITY : (k1 < bf) ? fmaf(__uint_as_float(v[i + 1]), p.scale_log2, nm) : u1;
-                    }
-                    mu = fmaxf(mu, fmaxf(u0, u1));
-                    const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
-                    rs_ += p0 + p1;
-                    pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
-                  }
-                }
-              }
-              store_chunks(sP + (c >> 6) * (kTile * 128) + row * 128, (c & 63) >> 3, pk);
-            }
-            rs_out = rs_;
-            return mu;
-          };
-          // Blocks after the first: ONE trip over the scores, relative to the running maximum (the block's own maximum is
-          // tracked on the way).  exp2(t - m_run) stays <= 2^8 unless a score exceeds every earlier one by more than 8
-          // (log2 units) — then, and only then, the warp redoes the block relative to the true maximum.  The softmax is
-          // the same function either way (numerator and denominator carry the same factor 2^(m_true - m_ref)).
-          const bool optimistic = __all_sync(0xffffffffu, j > 0 && m_run > kRealMax);
-          // (packed tiles: all_skip may differ between the rows of a warp, so the vote is taken by every lane; a skipped
-          // row has over = -inf, and a redo leaves it as it was: m_new = m_run, alpha = 1, P = 0)
-          if (optimistic) {
-            m_new = m_run;
-            alpha = 1.f;
-            rsum = 0.f;
-            float over = -INFINITY;
-            if (!all_skip) {
-              over = exp_pass(m_run, rsum);
-            } else {
-              float dummy;
-              exp_pass(m_run, dummy);   // (writes the zero P tile; no score reads: every chunk state is 0)
-            }
-            if (__any_sync(0xffffffffu, over > 8.0f)) {
-              m_new = fmaxf(m_run, m_run + over);
-              alpha = exp2f(m_run - m_new);
-              exp_pass(m_new, rsum);
-            }
-          } else {
-            // first block of an item (or no real key seen yet): pass 1 = row max (of the raw scores when `plain`:
-            // scale > 0 commutes with max), pass 2 = exp relative to it
-            float m_blk = -INFINITY;
-            if (!all_skip) {
-#pragma unroll 1
-              for (int c = 0; c < kTile; c += 32) {
-                const int sc_ = (stb >> (c >> 4)) & 3;
-                if (sc_ == 0) continue;
-                uint32_t v[32];
-                acc_ld_x32(srow + c, v);
-                if (plain) {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]));
-                } else if (sc_ == 1) {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]) * p.scale_log2);
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) {
-                    float t = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]);
-                    if (kPacked && (c + i < bl || c + i >= bh)) t = -INFINITY;
-                    m_blk = fmaxf(m_blk, t);
-                  }
+                for (int i = 0; i < 32; ++i) {
+                  float t = fmaf(__uint_as_float(v[i]), p.scale_log2, sbias[c + i]);
+                  if (kPacked && (c + i < bl || c + i >= bh)) t = -INFINITY;
+                  m_blk = fmaxf(m_blk, t);
                 }
               }
             }
-            if (plain) m_blk *= p.scale_log2;
-            m_new = fmaxf(m_run, m_blk);
-            alpha = (m_run == -INFINITY) ? 0.f : exp2f(m_run - m_new);
-            exp_pass(m_new, rsum);
           }
+          if (plain) m_blk *= p.scale_log2;
+          m_new = fmaxf(m_run, m_blk);
+          alpha = (m_run == -INFINITY) ? 0.f : exp2f(m_run - m_new);
+          exp_pass(m_new, rsum);
         }
         fence_proxy_async_smem();
         named_bar_sync(bar_id, kTile);   // P complete; every read of S is done
@@ -459,32 +404,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
           acc_store_frag(sS, Smem::kSPitch, 64, 0, o1);
         }
         named_bar_sync(bar_id, kTile);   // every row of O_blk is in the tile
-        if constexpr (kSingle) {
-          l_run = rsum;
-        } else {
-          if (!all_skip) {   // (a skipped block has P = 0: its O_blk is exactly 0 and alpha is exactly 1)
+        if (!all_skip) {   // (a skipped block has P = 0: its O_blk is exactly 0 and alpha is exactly 1)
 #pragma unroll
-            for (int c = 0; c < kDh; c += 32) {
-              uint32_t v[32];
-              acc_ld_x32(srow + c, v);
+          for (int c = 0; c < kDh; c += 32) {
+            uint32_t v[32];
+            acc_ld_x32(srow + c, v);
 #pragma unroll
-              for (int i = 0; i < 32; ++i) o[c + i] = fmaf(o[c + i], alpha, __uint_as_float(v[i]));
-            }
-            l_run = fmaf(l_run, alpha, rsum);
-            m_run = m_new;
+            for (int i = 0; i < 32; ++i) o[c + i] = fmaf(o[c + i], alpha, __uint_as_float(v[i]));
           }
+          l_run = fmaf(l_run, alpha, rsum);
+          m_run = m_new;
         }
       }
       // ctx tile = o / l in 16 bits: staged in this group's P buffer (the PV MMA has finished reading it), one TMA store
       {
         const float inv = 1.0f / l_run;
-        if constexpr (kSingle) {
-          uint32_t v[kDh];
-          acc_ld_x32(srow, v);
-          acc_ld_x32(srow + 32, v + 32);
-#pragma unroll
-          for (int i = 0; i < kDh; ++i) o[i] = __uint_as_float(v[i]);
-        }
 #pragma unroll
         for (int c = 0; c < kDh; c += 32) {
           uint32_t pk[16];
@@ -505,6 +439,285 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constan
     if (row == 0) bulk_wait_read_all();
   }
 
+}
+
+// =====================================================================================================================
+// Single key block: L <= 128 dense or packed (a tile holds 128 / L sequences), or a row plan whose sequences never
+// straddle a tile.  One work item = (128-row tile, head), the tile's own 128 rows as keys.
+//
+// Warp-specialised, persistent, one CTA of 384 threads per SM:
+//   warpgroup 0   producer: warp g (g = 0, 1) streams (Q, K, V) of consumer g's items into g's two-stage ring
+//   warpgroups 1, 2   consumers: consumer g walks its own items w = 2 blockIdx.x + g + n 2 gridDim.x, whole items each,
+//                 so that one consumer's softmax (MUFU / FMA) overlaps the other's wgmmas and loads
+// Per item a consumer runs, with S, P and O in registers (no fp32 tile in shared memory):
+//   S = Q K^T      wgmma m64n128k16 x (2 x 4), SS form (the same instructions and k order as the multi-block kernel)
+//   softmax        per row; thread t holds rows 16 (t/32) + (t%32)/4 + {0, 8, 64, 72} x keys 8 j + 2 (t%4) + {0, 1}
+//   O = P V        wgmma m64n64k16 x (2 x 8), RS form: the 16-bit S fragment, packed in pairs, is the A fragment
+//   ctx = O / l    16-bit, staged in the consumer's output tile, one TMA store
+// Bit-identical to the row-per-thread softmax this kernel replaced: a lane's 32 keys of a row are exactly the keys
+// (k >> 1) & 3 == t % 4 of that row's partial sum rs[(k >> 1) & 3] (pairs in rising order), and two xor shuffles (1,
+// then 2) form (rs0 + rs1) + (rs2 + rs3); maxima are exact in any order; P, and the key order of P V, are unchanged.
+struct SmemSingle {
+  static constexpr int kStages = 2;                                   // (Q, K, V) stages per consumer
+  static constexpr int kTileBytes = kTile * kDh * 2;                  // 16 KB
+  static constexpr int kStageBytes = 3 * kTileBytes;                  // Q at +0, K at +16 KB, V at +32 KB
+  static constexpr int kQKV = 0;                                      // [consumer][stage]
+  static constexpr int kOut = kQKV + 2 * kStages * kStageBytes;       // [consumer] 128 x 64 16-bit output tile
+  static constexpr int kBias = kOut + 2 * kTileBytes;                 // [consumer] 128 floats + 4 ballots
+  static constexpr int kBiasStride = kTile * 4 + 16;
+  static constexpr int kBar = kBias + 2 * kBiasStride;                // [consumer] full[kStages] empty[kStages]
+  static constexpr int kNumBars = 2 * 2 * kStages;
+  static constexpr int kTotal = kBar + kNumBars * 8;
+  static constexpr int kDynamic = kTotal + 1024;
+  static_assert(kDynamic <= 232448, "single-block attention smem exceeds 227 KB");
+};
+
+constexpr int kSingleThreads = 384;
+
+// Per-row state of the single-block softmax.  st: 2 bits per 32-key chunk (0 = every p is exactly 0, 1 = no key
+// masked, 2 = general); plain: max of the raw scores, scaled afterwards; [bl, bh): the row's own keys (kPacked).
+struct RowSt {
+  int st, bl, bh;
+  bool plain;
+};
+
+// Softmax of the two rows (r, r + 8) held by accumulator `d` (m64n128 fragment): P packed in pairs into `pk` (the A
+// fragments of the 8 k steps of P V), row sums (reduced over the quad) into rsum.
+template <bool kPacked, uint32_t FMT>
+__device__ __forceinline__ void softmax_pair(float (&d)[64], const RowSt& ra, const RowSt& rb, const float* sbias, int q4,
+                                             float scale_log2, uint32_t (&pk)[32], float& la, float& lb) {
+  const RowSt rs[2] = {ra, rb};
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = j >> 2;
+    const float2 b2 = *reinterpret_cast<const float2*>(sbias + 8 * j + 2 * q4);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const RowSt& r = rs[e >> 1];
+      const int col = 8 * j + 2 * q4 + (e & 1);
+      const int s = (r.st >> (2 * c)) & 3;
+      const float v = d[4 * j + e];
+      float t = fmaf(v, scale_log2, (e & 1) ? b2.y : b2.x);
+      if (kPacked && (col < r.bl || col >= r.bh)) t = -INFINITY;
+      t = r.plain ? v : (s == 1) ? v * scale_log2 : t;
+      d[4 * j + e] = t;
+      if (s != 0) mx[e >> 1] = fmaxf(mx[e >> 1], t);
+    }
+  }
+  float sc[2], nm[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float m = mx[i];
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    if (rs[i].plain) m *= scale_log2;
+    sc[i] = rs[i].plain ? scale_log2 : 1.0f;
+    nm[i] = -m;
+  }
+  float acc[2] = {0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = j >> 2;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {   // h: row r (d[4j], d[4j + 1]) or r + 8 (d[4j + 2], d[4j + 3])
+      const bool zero = ((rs[h].st >> (2 * c)) & 3) == 0;
+      const float p0 = zero ? 0.f : ex2_ftz(fmaf(d[4 * j + 2 * h], sc[h], nm[h]));
+      const float p1 = zero ? 0.f : ex2_ftz(fmaf(d[4 * j + 2 * h + 1], sc[h], nm[h]));
+      acc[h] += p0 + p1;
+      pk[2 * j + h] = act16::Act<FMT>::pack2(p0, p1);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {   // (rs0 + rs1) + (rs2 + rs3) on every lane of the quad
+    acc[i] = acc[i] + __shfl_xor_sync(0xffffffffu, acc[i], 1);
+    acc[i] = acc[i] + __shfl_xor_sync(0xffffffffu, acc[i], 2);
+  }
+  la = acc[0];
+  lb = acc[1];
+}
+
+template <bool kPacked, uint32_t FMT>
+__global__ void __launch_bounds__(kSingleThreads, 1)
+attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
+  using S = SmemSingle;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::kBar);   // consumer g: full at 2 kStages g, empty after it
+
+  // (broadcast from lane 0: ptxas then knows the warpgroup index, and every branch and loop bound derived from it, to
+  // be warp-uniform, and keeps the wgmmas of the consumer path pipelined)
+  const int wg = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);
+  const int n_tiles = (p.n_tokens + kTile - 1) / kTile;
+  const int total_work = n_tiles * p.heads;
+  const int stride = 2 * gridDim.x;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmCTX);
+    for (int g = 0; g < 2; ++g) {
+      for (int s = 0; s < S::kStages; ++s) {
+        mbar_init(bars + 2 * S::kStages * g + s, 1);
+        mbar_init(bars + 2 * S::kStages * g + S::kStages + s, 4);   // the four warps of consumer g, after P V
+      }
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ================================ TMA producers ================================
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp < 2 && lane == 0) {
+      uint64_t* full = bars + 2 * S::kStages * warp;
+      uint64_t* empty = full + S::kStages;
+      uint8_t* ring = smem + S::kQKV + warp * S::kStages * S::kStageBytes;
+      Ring<S::kStages> rq;
+      for (int w = 2 * blockIdx.x + warp; w < total_work; w += stride) {
+        const int tile = w / p.heads, h = w - tile * p.heads;
+        const int tok0 = tile * kTile;
+        mbar_wait(&empty[rq.stage], rq.phase ^ 1, 20);
+        mbar_arrive_expect_tx(&full[rq.stage], S::kStageBytes);
+        uint8_t* st = ring + rq.stage * S::kStageBytes;   // every byte is read once: evict first
+        tma_load_2d(st, &tmQKV, &full[rq.stage], h * kDh, tok0, kEvictFirst);
+        tma_load_2d(st + S::kTileBytes, &tmQKV, &full[rq.stage], p.hidden + h * kDh, tok0, kEvictFirst);
+        tma_load_2d(st + 2 * S::kTileBytes, &tmQKV, &full[rq.stage], 2 * p.hidden + h * kDh, tok0, kEvictFirst);
+        rq.advance();
+      }
+    }
+    return;
+  }
+
+  // ================================== consumers ==================================
+  const int g = wg - 1;
+  const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31, q4 = lane & 3;
+  const int r0 = 16 * warp + (lane >> 2);   // rows r0, r0 + 8 (accumulator 0) and r0 + 64, r0 + 72 (accumulator 1)
+  uint64_t* full = bars + 2 * S::kStages * g;
+  uint64_t* empty = full + S::kStages;
+  const uint32_t ring = smem_u32(smem + S::kQKV + g * S::kStages * S::kStageBytes);
+  uint8_t* sout = smem + S::kOut + g * S::kTileBytes;
+  float* sbias = reinterpret_cast<float*>(smem + S::kBias + g * S::kBiasStride);
+  unsigned* smask = reinterpret_cast<unsigned*>(sbias + kTile);   // per-warp ballots of masked keys
+  const int bar_id = 1 + g;
+  const bool varlen = kPacked && p.row_lo != nullptr;
+  Ring<S::kStages> rq;
+  // additive key bias of item w2 for key t of its tile (fetched one item ahead of its use)
+  auto load_bias = [&](int w2) -> float {
+    if (w2 >= total_work) return 0.f;
+    const int kt = (w2 / p.heads) * kTile + t;
+    return (kt < p.n_tokens) ? __ldg(p.kbias + kt) : -INFINITY;
+  };
+  float bv = load_bias(2 * blockIdx.x + g);
+  for (int w = 2 * blockIdx.x + g; w < total_work; w += stride) {
+    const int tile = w / p.heads, h = w - tile * p.heads;
+    const int tok0 = tile * kTile;
+    sbias[t] = bv;
+    {
+      const unsigned mk = __ballot_sync(0xffffffffu, bv < 0.f);
+      if (lane == 0) smask[warp] = mk;
+    }
+    if (t == 0) bulk_wait_read_all();   // the previous item's output tile has left sout
+    named_bar_sync(bar_id, kTile);
+    bv = load_bias(w + stride);
+    const unsigned mk[4] = {smask[0], smask[1], smask[2], smask[3]};
+    // Per row and 32-key chunk: 0 = every p is exactly 0 (keys of another packed sequence, or all keys masked while the
+    // row has an unmasked key somewhere: exp2(-10000 log2e + s - m) flushes to zero, as exp(-10000 + s - m) does in the
+    // reference's fp32 softmax), 1 = no key masked (no bias term), 2 = general.
+    RowSt rs[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int row = r0 + (i & 1) * 8 + (i >> 1) * 64;
+      int lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;   // keys of this row's own sequence
+      int hi = (p.L >= kTile) ? kTile : lo + p.L;
+      if (varlen) {
+        lo = __ldg(p.row_lo + tok0 + row) - tok0;
+        hi = __ldg(p.row_hi + tok0 + row) - tok0;
+      }
+      int st = 0;
+      if (varlen) {   // chunk outside / inside / straddling the boundary of the row's own sequence
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          st |= ((hi <= c * 32 || lo >= c * 32 + 32) ? 0 : (lo <= c * 32 && hi >= c * 32 + 32) ? 1 : 2) << (2 * c);
+      } else {
+        bool own[4], any_unmasked = false;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          own[c] = !kPacked || (p.L >= 32 ? (c * 32 >= lo && c * 32 < hi) : c == (row >> 5));
+          any_unmasked |= own[c] && mk[c] != 0xffffffffu;
+        }
+        const bool skip_ok = (kPacked && p.L < 32) ? false : any_unmasked;
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          st |= (!own[c] ? 0 : (mk[c] == 0xffffffffu && skip_ok) ? 0 : (mk[c] == 0u && !(kPacked && p.L < 32)) ? 1 : 2)
+                << (2 * c);
+      }
+      rs[i].st = st;
+      rs[i].bl = lo;
+      rs[i].bh = hi;
+      rs[i].plain = kPacked ? (varlen && lo <= 0 && hi >= kTile) : ((mk[0] | mk[1] | mk[2] | mk[3]) == 0u);
+    }
+
+    mbar_wait(&full[rq.stage], rq.phase, 21);
+    const uint32_t sq = ring + rq.stage * S::kStageBytes, sk = sq + S::kTileBytes, sv = sq + 2 * S::kTileBytes;
+    // One 64-row half at a time: S = Q K^T, its softmax, O = P V (keys in the order of the multi-block kernel: 8 steps
+    // of 16), then ctx = O / l in 16 bits into the output tile (SWIZZLE_128B: 16-byte chunk index ^= row & 7).  The P V
+    // of half 0 is issued before the S of half 1, and wgmmas issue in program order, so the S of half 1 cannot be
+    // hoisted above the softmax of half 0: one half of S, P and O is live at a time, and nothing spills.  (The other
+    // consumer warpgroup covers the waits.)
+    auto half = [&](int m0, const RowSt& ra, const RowSt& rb) {
+      uint32_t pk[32];
+      float l[2];
+      {
+        float s[kTile / 2];
+#pragma unroll
+        for (int i = 0; i < kTile / 2; ++i) s[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kDh / 16; ++k)
+          wgmma_n128<FMT, 0>(s, make_desc_k_sw128(sq + m0 * 128 + k * 32), make_desc_k_sw128(sk + k * 32), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        softmax_pair<kPacked, FMT>(s, ra, rb, sbias, q4, p.scale_log2, pk, l[0], l[1]);
+      }
+      float o[kDh / 2];
+#pragma unroll
+      for (int i = 0; i < kDh / 2; ++i) o[i] = 0.f;
+      wgmma_fence_regs(pk);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kTile / 16; ++k) {
+        const uint32_t a[4] = {pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]};
+        wgmma_n64_rs<FMT>(o, a, make_desc_mn_sw128(sv + k * 2048, kTile * 128, 1024));   // 16 keys: two 8-row groups
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {   // rows m0 + r0 + 8 hh: o[4 j + 2 hh + 0..1], keys 8 j + 2 (t % 4) + 0..1
+        const int row = m0 + r0 + 8 * hh;
+        const float inv = 1.0f / l[hh];
+        uint8_t* rowp = sout + row * 128 + q4 * 4;
+#pragma unroll
+        for (int j = 0; j < kDh / 8; ++j) {
+          const int e = 4 * j + 2 * hh;
+          *reinterpret_cast<uint32_t*>(rowp + ((j ^ (row & 7)) << 4)) = act16::Act<FMT>::pack2(o[e] * inv, o[e + 1] * inv);
+        }
+      }
+    };
+    half(0, rs[0], rs[1]);
+    half(64, rs[2], rs[3]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[rq.stage]);   // this warp's last read of the stage
+    rq.advance();
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, kTile);
+    if (t == 0) {
+      tma_store_2d(&tmCTX, sout, h * kDh, tok0);   // rows past n_tokens are clipped by the tensor map
+      bulk_commit_group();
+    }
+  }
+  if (t == 0) bulk_wait_read_all();
 }
 
 }  // namespace attn

@@ -573,10 +573,10 @@ int layer_norm(const void* in, bool in_f32, size_t in_ld, int rows, int H, const
 template <uint32_t FMT>
 int set_attention_attrs() {
   // per device, not per process: a second GPU used from the same process needs its own opt-in
-  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<false, false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
-  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<false, true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
-  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<true, true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
-  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_kernel<true, false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   return ANCE_OK;
 }
 
@@ -587,7 +587,7 @@ struct AttentionLaunch {
   CUtensorMap tmQKV, tmCTX;
   attn::Params ap;
   int grid;
-  bool packed, single;   // the attention_kernel<kPacked, kSingle> instantiation
+  bool packed, single;   // attention_single_kernel<kPacked> (one key block per item) or attention_multi_kernel<kPacked>
 };
 
 int make_attention(AttentionLaunch& a, const uint16_t* qkv, uint16_t* ctx, int n_tokens, int L, int heads,
@@ -611,19 +611,20 @@ int make_attention(AttentionLaunch& a, const uint16_t* qkv, uint16_t* ctx, int n
   ap.row_hi = varlen ? row_hi : nullptr;
   ap.tile_kv = varlen ? tile_kv : nullptr;
   const int attn_work = ((n_tokens + 127) / 128) * heads;
-  a.grid = std::min(attn_work, gemm::sm_count());
   a.packed = varlen || L < attn::kTile;
   a.single = !varlen_long && L <= attn::kTile;
+  // the single-block kernel takes two items at a time per CTA (one per MMA warpgroup)
+  a.grid = std::min(a.single ? (attn_work + 1) / 2 : attn_work, gemm::sm_count());
   return ANCE_OK;
 }
 
 template <uint32_t FMT>
 int run_attention(const AttentionLaunch& a, cudaStream_t st) {
   ance::prof_begin(ance::kClsAttn, st);
-  if (a.packed && !a.single) attn::attention_kernel<true, false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
-  else if (a.packed) attn::attention_kernel<true, true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
-  else if (a.single) attn::attention_kernel<false, true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
-  else attn::attention_kernel<false, false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  if (a.single && a.packed) attn::attention_single_kernel<true, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else if (a.single) attn::attention_single_kernel<false, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else if (a.packed) attn::attention_multi_kernel<true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  else attn::attention_multi_kernel<false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   ance::prof_end(ance::kClsAttn, st);
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);

@@ -235,6 +235,31 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64
   else wgmma_m64n64k16_f16<kTransB>(d, adesc, bdesc, accumulate);
 }
 
+// D += A[registers] * B[smem], m64n64k16, B MN-major.  A fragment (4 x 32-bit, two 16-bit values each, low half = lower
+// k): thread t holds rows 16 (t/32) + (t%32)/4 (+8) and k = 2 (t%4) + 0..1 (+8), i.e. a[0] = (row, k), a[1] = (row + 8,
+// k), a[2] = (row, k + 8), a[3] = (row + 8, k + 8): the accumulator fragment of an m64nN tile, columns [16 s, 16 s + 16),
+// packed in pairs, is the A fragment of k step s.
+#define TC05_WGMMA_RS(NAME, INSTR)                                                                                    \
+  __device__ __forceinline__ void NAME(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {                     \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t" INSTR " {" TC05_S32                              \
+                 "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"                                                     \
+                 : TC05_R32                                                                                           \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1u));                                  \
+  }
+TC05_WGMMA_RS(wgmma_m64n64k16_rs_bf16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16")
+TC05_WGMMA_RS(wgmma_m64n64k16_rs_f16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16")
+template <uint32_t FMT>
+__device__ __forceinline__ void wgmma_n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  if constexpr (FMT == kFmtBF16) wgmma_m64n64k16_rs_bf16(d, a, bdesc);
+  else wgmma_m64n64k16_rs_f16(d, a, bdesc);
+}
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t (&a)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+
 // ----------------------------------------------------------------------------------------------
 // accumulator tiles in shared memory: fp32, row-major, `pitch` words per row (pitch % 32 == 4: the
 // row-per-thread reads below are free of bank conflicts).  The wgmma fragment of rows [r0, r0 + 64) is
