@@ -133,7 +133,12 @@ SIGNATURES = {
     "ance_dbg_transpose_bf16": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p]),
     "ance_dbg_train_layout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ance_dbg_index_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
 }
+
+# ance_dbg_index_state's items (ANCE_STATE_*), in order
+INDEX_STATE_ITEMS = ("mu", "centred", "p16", "pstats", "ndelta", "q16", "qn_hat", "qn_delta", "cand_id", "cand_cnt",
+                     "cand_thr", "pass", "flagged", "flagged_cnt", "flagged_thr")
 
 # ance_dbg_train_layout's fields, in order
 TRAIN_LAYOUT_FIELDS = ("ids", "kbias", "layers", "per_layer", "x_in", "qkv", "ctx", "t1", "x1", "u", "ff", "t2",
@@ -178,6 +183,16 @@ def ptr(t) -> int:
 def current_stream() -> int:
     import torch
     return torch.cuda.current_stream().cuda_stream
+
+
+def index_state(handle, item: str, out) -> None:
+    """ance_dbg_index_state: copy `item` (one of INDEX_STATE_ITEMS) of an index handle into `out`, a contiguous torch
+    tensor (CPU or CUDA) or numpy array whose size in bytes is the item's exact size (else AnceError)."""
+    if hasattr(out, "data_ptr"):
+        dst, nbytes = out.data_ptr(), out.numel() * out.element_size()
+    else:
+        dst, nbytes = out.ctypes.data, out.nbytes
+    check(load().ance_dbg_index_state(handle, INDEX_STATE_ITEMS.index(item), dst, nbytes, current_stream()))
 
 
 PROFILE_CLASSES = ("gemm_head", "attention", "norm_embed", "quantize", "coarse_search", "rescore", "exact",

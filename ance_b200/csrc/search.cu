@@ -999,6 +999,12 @@ struct ance_index {
   // last search
   ance_search_stats stats{};
   cudaStream_t last_stream = nullptr;
+  // what ance_dbg_index_state may copy: the query block of the last search_tiers (0: none), its tier-1 flagged count,
+  // and the shape of the last coarse pass (tier 1, or tier 2 when one ran after it)
+  int64_t dbg_q_n = 0;
+  int dbg_flagged1 = 0;
+  int dbg_pass_nq = 0, dbg_pass_ns = 0, dbg_pass_out_cap = 0, dbg_pass_kprime = 0, dbg_pass_rows_per_split = 0,
+      dbg_pass_tier = 0;
 };
 
 namespace {
@@ -1062,6 +1068,7 @@ int launch_coarse(ance_index* ix, const uint16_t* Q16, int64_t nq, int kprime, i
   const int N = static_cast<int>(ix->n);
   gemm::WorkShape ws = gemm::make_shape(static_cast<int>(nq), N, ix->dim, BN, CG, n_splits_req);
   *n_splits_out = ws.n_splits;
+  ix->dbg_pass_rows_per_split = ws.n_blks_per_split * BN;   // split s covers rows [s, s + 1) * this
   // One sweep per query tile: every concurrently running CTA pair re-reads the same corpus tile, so keep it in L2.
   // With row-range splits each pair streams its own range once: do not let it evict the (re-read) query tiles.
   ws.hint_b = (ws.n_splits == 1) ? tc05::kEvictNormal : tc05::kEvictFirst;
@@ -1298,6 +1305,11 @@ int coarse_rescore_pass(ance_index* ix, const uint16_t* Q16, const float* q_f32,
 #undef ANCE_COARSE
   if (rc) return rc;
   *ns_out = ns;
+  ix->dbg_pass_nq = static_cast<int>(nq);
+  ix->dbg_pass_ns = ns;
+  ix->dbg_pass_out_cap = out_cap;
+  ix->dbg_pass_kprime = kprime;
+  ix->dbg_pass_tier = thr_init ? 2 : 1;
   RescoreParams rp;
   rp.Q = q_f32;
   rp.P = ix->P32;
@@ -1528,6 +1540,7 @@ int search_tiers(ance_index* ix, const float* q_dev, int64_t nq, int k, int kpri
     ix->flagged_cap = f;
   }
   ANCE_CUDA(cudaMemsetAsync(ix->counters, 0, kCntRowErr * sizeof(int), st));   // everything but the sticky row flag
+  ix->dbg_q_n = nq;
   const unsigned qblocks = static_cast<unsigned>((nq + 7) / 8);
   ance::prof_begin(ance::kClsQuant, st);
   if (ix->fmt == ANCE_FMT_BF16)
@@ -1556,6 +1569,7 @@ int search_tiers(ance_index* ix, const float* q_dev, int64_t nq, int k, int kpri
     return ANCE_ERR_UNSUPPORTED;
   }
   int n_exact = h[0];
+  ix->dbg_flagged1 = h[0];
   int ns2 = 0;
   if (h[0] > 0 && ix->tier2 && ix->n >= 4 * static_cast<int64_t>(tier2_kprime)) {
     // --- tier 2: the uncertified queries once more, from their own thresholds (nothing that passes is dropped)
@@ -1719,6 +1733,9 @@ extern "C" int ance_index_search(ance_index_t ix, const float* q_dev, int64_t nq
   if (rc) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   ix->last_fetched = 0;
+  ix->dbg_q_n = 0;       // until search_tiers runs (the brute-force route below never does)
+  ix->dbg_pass_nq = 0;
+  ix->dbg_flagged1 = 0;
   // choose k' (candidates kept per split).  The certificate needs every row within eps of the k-th score among the
   // candidates; eps is ~0.5 (fp16 operands) / ~3 (bf16) for rows of norm 27.7, i.e. ~0.1 k / ~0.6 k extra rows on the
   // distributions of tools/exp_certify.py.  A query that k' does not cover costs one tier-2 pass, not a wrong answer.
@@ -1787,3 +1804,52 @@ extern "C" int ance_index_memory(ance_index_t ix, int64_t* device_bytes, int64_t
 extern "C" int64_t ance_index_last_fetched(ance_index_t ix) { return ix ? ix->last_fetched : -1; }
 
 extern "C" float* ance_index_host_rows(ance_index_t ix) { return (ix && ix->host_rows) ? ix->P32_host : nullptr; }
+
+extern "C" int ance_dbg_index_state(ance_index_t ix, int what, void* dst, int64_t n_bytes, void* stream) {
+  ANCE_REQUIRE(ix != nullptr, "ance_dbg_index_state: null handle");
+  int rc = check_handle_device(ix, "ance_dbg_index_state");
+  if (rc) return rc;
+  const int64_t n = ix->n, d = ix->dim;
+  const int64_t slots = static_cast<int64_t>(ix->dbg_pass_nq) * ix->dbg_pass_ns;
+  const bool rows = ix->n > 0 && !ix->dirty;   // the 16-bit operands match the rows
+  const void* src = nullptr;
+  int64_t want = -1;
+  int32_t host[6] = {};
+  switch (what) {
+    case ANCE_STATE_MU: src = ix->mu; want = rows ? d * 4 : -1; break;
+    case ANCE_STATE_CENTRED: host[0] = ix->centred; src = host; want = rows ? 4 : -1; break;
+    case ANCE_STATE_P16: src = ix->P16; want = rows ? n * d * 2 : -1; break;
+    case ANCE_STATE_PSTATS: src = ix->pstats; want = rows ? 8 : -1; break;
+    case ANCE_STATE_NDELTA: src = ix->ndelta; want = (rows && ix->host_rows) ? n * 4 : -1; break;
+    case ANCE_STATE_Q16: src = ix->Q16; want = ix->dbg_q_n ? ix->dbg_q_n * d * 2 : -1; break;
+    case ANCE_STATE_QN_HAT: src = ix->qn_hat; want = ix->dbg_q_n ? ix->dbg_q_n * 4 : -1; break;
+    case ANCE_STATE_QN_DELTA: src = ix->qn_delta; want = ix->dbg_q_n ? ix->dbg_q_n * 4 : -1; break;
+    case ANCE_STATE_CAND_ID: src = ix->cand_id; want = slots ? slots * ix->dbg_pass_out_cap * 4 : -1; break;
+    case ANCE_STATE_CAND_CNT: src = ix->cand_cnt; want = slots ? slots * 4 : -1; break;
+    case ANCE_STATE_CAND_THR: src = ix->cand_thr; want = slots ? slots * 4 : -1; break;
+    case ANCE_STATE_PASS:
+      host[0] = ix->dbg_pass_nq;
+      host[1] = ix->dbg_pass_ns;
+      host[2] = ix->dbg_pass_out_cap;
+      host[3] = ix->dbg_pass_kprime;
+      host[4] = ix->dbg_pass_rows_per_split;
+      host[5] = ix->dbg_pass_tier;
+      src = host;
+      want = slots ? 24 : -1;
+      break;
+    case ANCE_STATE_FLAGGED: src = ix->flagged; want = ix->dbg_q_n ? int64_t(ix->dbg_flagged1) * 4 : -1; break;
+    case ANCE_STATE_FLAGGED_CNT: host[0] = ix->dbg_flagged1; src = host; want = ix->dbg_q_n ? 4 : -1; break;
+    case ANCE_STATE_FLAGGED_THR: src = ix->flagged_thr; want = ix->dbg_q_n ? int64_t(ix->dbg_flagged1) * 4 : -1; break;
+    default: ance::set_error("ance_dbg_index_state: unknown item %d", what); return ANCE_ERR_INVALID;
+  }
+  ANCE_REQUIRE(want >= 0, "ance_dbg_index_state: item %d is not held (no search since the index changed, or not a host index)",
+               what);
+  ANCE_REQUIRE(n_bytes == want, "ance_dbg_index_state: item %d has %lld bytes, not %lld", what, (long long)want,
+               (long long)n_bytes);
+  if (want == 0) return ANCE_OK;   // an empty flagged list
+  ANCE_REQUIRE(dst != nullptr, "ance_dbg_index_state: dst is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ANCE_CUDA(cudaMemcpyAsync(dst, src, static_cast<size_t>(want), cudaMemcpyDefault, st));
+  ANCE_CUDA(cudaStreamSynchronize(st));   // `host` is a local
+  return ANCE_OK;
+}

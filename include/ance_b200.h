@@ -354,6 +354,26 @@ int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, i
  * u, ff [., ffn].  In the pruned last layer T1, X1, U, FF and T2 are compact: row b is sequence b's CLS row (B rows used);
  * CTX keeps its B * L rows (the CLS rows are read at pitch L * hidden); X_in and QKV are full. */
 int ance_dbg_train_layout(ance_encoder_t enc, int B, int L, size_t* out);
+/* Read-only copy of what a flat-IP index holds for the exactness certificate, into dst (host or device memory; the
+ * stream is synchronised).  n_bytes must be the item's exact size, else ANCE_ERR_INVALID, as is an item the index does
+ * not hold (no search since rows were added or the format changed; ndelta of a device index).  Items:
+ *   rows (after the last prepare / search): MU fp32 [dim] (the centre; meaningful when CENTRED), CENTRED int32,
+ *     P16 [n, dim] 16-bit operand rows, PSTATS [2] fp32 bits (max ||p^||, max ||p - mu - p^||), NDELTA fp32 [n] (host
+ *     index: per-row ||p - mu - p^||, rounded up);
+ *   the last ance_index_search's queries (its last block of <= 16,384 when k > 512): Q16 [nq, dim], QN_HAT, QN_DELTA fp32
+ *     [nq]; the tier-1 uncertified list FLAGGED int32 [cnt] in slot order, FLAGGED_CNT int32, FLAGGED_THR fp32 [cnt]
+ *     (tier 2's starting threshold of each slot);
+ *   the last coarse pass (tier 1, or tier 2 when it ran; slot = query * n_splits + split, a tier-2 query is
+ *     FLAGGED[query]): CAND_ID int32 [slots, out_cap], CAND_CNT int32 [slots], CAND_THR fp32 [slots] (every row of the
+ *     split that is not a candidate has coarse score <= it), PASS int32 [6] = nq, n_splits, out_cap, k', rows per split
+ *     (split s covers rows [s * it, (s + 1) * it)), tier. */
+enum {
+  ANCE_STATE_MU = 0, ANCE_STATE_CENTRED = 1, ANCE_STATE_P16 = 2, ANCE_STATE_PSTATS = 3, ANCE_STATE_NDELTA = 4,
+  ANCE_STATE_Q16 = 5, ANCE_STATE_QN_HAT = 6, ANCE_STATE_QN_DELTA = 7, ANCE_STATE_CAND_ID = 8, ANCE_STATE_CAND_CNT = 9,
+  ANCE_STATE_CAND_THR = 10, ANCE_STATE_PASS = 11, ANCE_STATE_FLAGGED = 12, ANCE_STATE_FLAGGED_CNT = 13,
+  ANCE_STATE_FLAGGED_THR = 14
+};
+int ance_dbg_index_state(ance_index_t idx, int what, void* dst, int64_t n_bytes, void* stream);
 
 #ifdef __cplusplus
 }
