@@ -5,11 +5,12 @@
     18,944 at k = 1000.  Per case and mode: ms per search (CUDA events, mean of --iters), device ms of the coarse pass
     and of the rescoring (ance_profile_read, a separate profiled search), candidates rescored, rows fetched from host
     memory, the GB they make and the PCIe rate that implies over the host rescoring's device time, memory() of both
-    indexes, and torch.equal of D and I between the modes.  Also the host index's add (D2H) and prepare (H2D) times.
+    indexes, torch.equal of D and I between the modes, and the first and last 32 queries of every query block (k > 512:
+    blocks of at most 16,384) of the host index's answer against its exact=True.  Also the host index's add (D2H) and prepare (H2D) times.
 (b) A host index of 21,015,324 rows (DPR's corpus), generated on the GPU in blocks and added block by block: add and
     prepare time, searches at DPR's shapes (58,880 queries at k = 200; 3,610 and 11,313 at k = 100), memory(), and the
-    first 64 queries compared bit for bit with exact=True (the brute force copies the rows H2D once per query batch),
-    with the time that takes.  Skipped, with the reason, when MemAvailable is below the 65 GB of pinned rows it needs.
+    first and last 32 queries of every query block compared bit for bit with exact=True (the brute force copies the rows
+    H2D once per query batch), with the time that takes.  Skipped, with the reason, when MemAvailable is below the 65 GB of pinned rows it needs.
 The card's name, power limit and SM clock are read in the same run.  One JSON line per record.
 
     python tools/bench_host_rows.py [--iters 2] [--parts ab] [--out FILE]
@@ -26,7 +27,7 @@ import torch  # noqa: E402
 
 from ance_b200 import _lib  # noqa: E402
 from ance_b200.search import IndexFlatIP  # noqa: E402
-from tools.bench_large_k import gpu_info  # noqa: E402
+from tools.bench_large_k import block_edges, equals_exact, gpu_info  # noqa: E402
 from tools.bringup_search import make_data  # noqa: E402
 
 D = 768
@@ -104,6 +105,8 @@ def part_a(a, dev, out):
         Dh, Ih = hi.search_device(q, k)
         sth, fetched = hi.stats(), hi.last_fetched()
         prof_d, prof_h = profiled(di, q, k), profiled(hi, q, k)
+        edges = block_edges(nq, k)
+        exact_ok = equals_exact(hi, q, k, Dh, Ih, edges)
         fetched_gb = fetched * D * 4 / 1e9
         emit({"part": "a", "rows": ROWS_A, "nq": nq, "k": k, "operand": "fp16",
               "device_ms": round(sum(ms["device"]) / len(ms["device"]), 3),
@@ -114,7 +117,8 @@ def part_a(a, dev, out):
               "fetched_rows": fetched, "fetched_GB": round(fetched_gb, 3),
               "implied_pcie_GBps": round(fetched_gb / (prof_h["rescore"] / 1e3), 1) if prof_h["rescore"] else None,
               "memory_device_index": di.memory(), "memory_host_index": hi.memory(),
-              "equal_D_I": bool(torch.equal(Dd, Dh) and torch.equal(Id, Ih)), "gpu": gpu_info()}, out)
+              "equal_D_I": bool(torch.equal(Dd, Dh) and torch.equal(Id, Ih)), "exact_block_edges": len(edges),
+              "exact_block_edges_bitexact": exact_ok, "gpu": gpu_info()}, out)
     del di, hi, P, Q
     torch.cuda.empty_cache()
 
@@ -156,17 +160,17 @@ def part_b(a, dev, out):
         ms, Dh, Ih = search_ms(hi, q, k, 1)
         st, fetched = hi.stats(), hi.last_fetched()
         prof = profiled(hi, q, k)
+        edges = block_edges(nq, k)
         res = {}
-        t_exact = timed(lambda: res.update(DI=hi.search_device(q[:64], k, exact=True)))
-        De, Ie = res["DI"]
-        ok = bool(torch.equal(Ie, Ih[:64]) and torch.equal(De.view(torch.int32), Dh[:64].view(torch.int32)))
+        t_exact = timed(lambda: res.update(ok=equals_exact(hi, q, k, Dh, Ih, edges)))
         fetched_gb = fetched * D * 4 / 1e9
         emit({"part": "b", "rows": ROWS_B, "nq": nq, "k": k, "operand": "fp16", "host_ms": round(ms, 3),
               "qps": round(nq / ms * 1e3, 1), "kernel_ms": prof, "n_candidates": st["n_candidates"],
               "n_splits": st["n_splits"], "n_tier2": st["n_tier2"], "n_uncertified": st["n_uncertified"],
               "fetched_rows": fetched, "fetched_GB": round(fetched_gb, 3),
               "implied_pcie_GBps": round(fetched_gb / (prof["rescore"] / 1e3), 1) if prof["rescore"] else None,
-              "memory": hi.memory(), "exact_64_s": round(t_exact, 3), "exact_slice_64_bitexact": ok, "gpu": gpu_info()}, out)
+              "memory": hi.memory(), "exact_block_edges": len(edges), "exact_block_edges_s": round(t_exact, 3),
+              "exact_block_edges_bitexact": res["ok"], "gpu": gpu_info()}, out)
 
 
 def main():

@@ -7,8 +7,9 @@ One JSON line per case:
 Per case: ms per search and queries/s (CUDA events, mean of --iters searches after a warm-up), the search statistics
 (kprime, n_splits, n_tier2, n_uncertified, n_candidates), device ms per kernel class from ance_profile_read (a separate
 profiled search), the workspace the search allocated (device memory in use after its first search on a fresh index
-minus before), and bit-exact agreement of the first 64 queries with search_device(..., exact=True).  The card's name,
-power limit and SM clock are read in the same run.
+minus before), and bit-exact agreement with search_device(..., exact=True) of the first and last 32 queries of every
+query block (k > 512: blocks of at most 16,384; otherwise the call is one block).  The card's name, power limit and SM
+clock are read in the same run.
 
     python tools/bench_large_k.py [--rows 8841823] [--iters 3] [--out FILE]
 """
@@ -27,6 +28,28 @@ from ance_b200.search import IndexFlatIP  # noqa: E402
 from tools.bringup_search import make_data  # noqa: E402
 
 CASES = [(6980, 100), (6980, 1000), (18944, 200), (18944, 500), (18944, 1000), (18944, 2048)]
+WIDE_QBLOCK = 16384   # search.cu kWideQBlock
+
+
+def block_edges(nq, k, edge=32):
+    """Query numbers of the first and last `edge` queries of every block ance_index_search splits nq into (k > 512:
+    equal blocks of at most 16,384 rounded up to the 256-query tile; otherwise one block)."""
+    qb = nq
+    if k > 512:
+        n_blocks = -(-nq // WIDE_QBLOCK)
+        qb = min(WIDE_QBLOCK, -(-(-(-nq // n_blocks)) // 256) * 256)
+    rows = set()
+    for b0 in range(0, nq, qb):
+        b1 = min(nq, b0 + qb)
+        rows |= set(range(b0, min(b1, b0 + edge))) | set(range(max(b0, b1 - edge), b1))
+    return sorted(rows)
+
+
+def equals_exact(idx, q, k, D, I, rows):
+    """D / I of `rows` bit for bit equal to the brute force's answer for those queries."""
+    r = torch.as_tensor(rows, device=q.device)
+    De, Ie = idx.search_device(q[r].contiguous(), k, exact=True)
+    return bool(torch.equal(Ie, I[r]) and torch.equal(De.view(torch.int32), D[r].view(torch.int32)))
 
 
 def gpu_info():
@@ -78,21 +101,21 @@ def main():
         idx.search_device(q, k)
         prof = _lib.profile_read(reset=True)
         _lib.profile_enable(False)
-        De, Ie = idx.search_device(q[:64], k, exact=True)
-        torch.cuda.synchronize()
-        exact_ok = bool((Ie == I[:64]).all().item() and (De.view(torch.int32) == D[:64].view(torch.int32)).all().item())
+        edges = block_edges(nq, k)
+        exact_ok = equals_exact(idx, q, k, D, I, edges)
         rec = {"case": "dev-small" if nq == 6980 else "driver-block", "rows": a.rows, "nq": nq, "k": k, "operand": "fp16",
                "ms": round(ms, 3), "qps": round(nq / ms * 1e3, 1),
                "kprime": st["kprime"], "n_splits": st["n_splits"], "n_tier2": st["n_tier2"],
                "n_uncertified": st["n_uncertified"], "n_candidates": st["n_candidates"],
                "device_ms": {c: round(prof[c][0], 3) for c in ("quantize", "coarse_search", "rescore", "exact")},
-               "workspace_bytes": int(workspace), "exact_slice_64_bitexact": exact_ok, "gpu": info}
+               "workspace_bytes": int(workspace), "exact_block_edges": len(edges), "exact_block_edges_bitexact": exact_ok,
+               "gpu": info}
         line = json.dumps(rec)
         print(line, flush=True)
         if out:
             out.write(line + "\n")
             out.flush()
-        del idx, D, I, De, Ie
+        del idx, D, I
         torch.cuda.empty_cache()
 
 
