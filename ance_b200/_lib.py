@@ -125,6 +125,8 @@ SIGNATURES = {
                                       C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "ance_dbg_attention_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                               C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_dbg_attention_backward_long": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                   C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ance_dbg_layer_norm_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                                C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p]),

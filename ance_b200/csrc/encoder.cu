@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "attention.cuh"
+#include "attn_bwd_long.cuh"
 #include "common.h"
 #include "encoder_bwd.cuh"
 #include "gemm_store.cuh"
@@ -441,6 +442,7 @@ struct ance_encoder {
   std::vector<void*> allocs;
   // training (ance_encoder_forward_train / _backward)
   std::map<const void*, int2> train_shapes;   // workspace -> (B, L) of a forward_train whose backward has not run yet
+  int train_max_len = 128;                    // ance_encoder_set_param("train_max_len"): longest L the training calls accept
   struct LayerT { uint16_t *wqkv, *wo, *w1, *w2; };   // bf16 W^T: [H,3H] [H,H] [H,F] [F,H]
   std::vector<LayerT> wt;                     // empty until the first backward
   uint16_t* head_wt = nullptr;
@@ -680,7 +682,7 @@ struct TrainSave {
 
 // n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
 // token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
-// ts != null (dense, L <= 128): the training forward — the same launches on the same inputs, with every activation the
+// ts != null (dense, L <= the handle's train_max_len): the training forward — the same launches on the same inputs, with every activation the
 // backward needs written to its own slot of the workspace instead of the reused buffers of the handle (plus the FFN-up
 // GEMM once more without GELU for the pre-activation), and the last layer always pruned to the CLS rows.
 template <uint32_t FMT>
@@ -981,6 +983,19 @@ int attn_bwd(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool
   return ANCE_OK;
 }
 
+// L in {256, 384, 512}: the key-blocked kernels of attn_bwd_long.cuh; stats: bwdl::stats_floats(B, L, heads) fp32
+template <uint32_t FMT>
+int attn_bwd_long(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, float* stats,
+                  int B, int L, int heads, cudaStream_t st) {
+  const dim3 grid(L / bwdl::kBlk, heads, B);
+  ance::ProfScope ps(ance::kClsAttn, st);
+  bwdl::dq_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f);
+  bwdl::dkv_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(2);
+  return ANCE_OK;
+}
+
 // bf16 W^T copies of every linear weight (dgrad operands), rebuilt from the 16-bit weights after a change
 template <uint32_t FMT>
 int ensure_wt(ance_encoder* e, cudaStream_t st) {
@@ -1021,14 +1036,16 @@ struct BwdScratch {
   float *G, *dT, *dA, *dX1, *part;
   uint16_t *A16, *Gt, *Xt, *dCTX;
   int32_t* pos;
+  float* attn_stats;   // [B * heads, 3, L]: per-row softmax statistics of the L > 128 attention backward
 };
 
 int ensure_scratch(ance_encoder* e, int M, BwdScratch& s) {
   const size_t H = e->cfg.hidden, F = e->cfg.ffn, N = std::max(3 * H, F), Mp = (M + 7) / 8 * 8;
   auto up = [](size_t x) { return (x + 255) / 256 * 256; };
   const size_t part = std::max(static_cast<size_t>(bwd::kLnBwdMaxBlocks) * 3 * H, static_cast<size_t>(bwd::kColsumChunks) * N);
-  const size_t sz[10] = {up(M * H * 4), up(M * H * 4), up(M * N * 4), up(M * H * 4), up(part * 4),
-                         up(M * N * 2), up(N * Mp * 2), up(N * Mp * 2), up(M * H * 2), up(static_cast<size_t>(M) * 4)};
+  const size_t sz[11] = {up(M * H * 4), up(M * H * 4), up(M * N * 4), up(M * H * 4), up(part * 4),
+                         up(M * N * 2), up(N * Mp * 2), up(N * Mp * 2), up(M * H * 2), up(static_cast<size_t>(M) * 4),
+                         up(bwdl::stats_floats(1, M, e->cfg.heads) * 4)};
   size_t total = 0;
   for (size_t x : sz) total += x;
   if (total > e->bwd_scratch_bytes) {
@@ -1043,12 +1060,13 @@ int ensure_scratch(ance_encoder* e, int M, BwdScratch& s) {
     e->bwd_scratch_bytes = total;
   }
   uint8_t* p = reinterpret_cast<uint8_t*>(e->bwd_scratch);
-  void* q[10];
-  for (int i = 0; i < 10; ++i) { q[i] = p; p += sz[i]; }
+  void* q[11];
+  for (int i = 0; i < 11; ++i) { q[i] = p; p += sz[i]; }
   s.G = static_cast<float*>(q[0]); s.dT = static_cast<float*>(q[1]); s.dA = static_cast<float*>(q[2]);
   s.dX1 = static_cast<float*>(q[3]); s.part = static_cast<float*>(q[4]);
   s.A16 = static_cast<uint16_t*>(q[5]); s.Gt = static_cast<uint16_t*>(q[6]); s.Xt = static_cast<uint16_t*>(q[7]);
   s.dCTX = static_cast<uint16_t*>(q[8]); s.pos = static_cast<int32_t*>(q[9]);
+  s.attn_stats = static_cast<float*>(q[10]);
   return ANCE_OK;
 }
 
@@ -1122,7 +1140,9 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     if ((rc = wgrad(s.Gt, H, s.Xt, H, Mrp, lg.ao_w, st))) return rc;
     if ((rc = linear<kBF>(s.A16, H, Mr, wt.wo, H, H, nullptr, nullptr, 0, s.dCTX, nullptr, st))) return rc;  // d CTX (bf16)
     // attention -> d QKV [M, 3H]
-    if ((rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st))) return rc;
+    if (L <= attn::kTile) rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st);
+    else rc = attn_bwd_long<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, s.attn_stats, B, L, c.heads, st);
+    if (rc) return rc;
     if ((rc = colsum(s.dA, M, 3 * H, s.part, H, lg.q_b, lg.k_b, lg.v_b, st))) return rc;
     if ((rc = to_bf16(s.dA, s.A16, static_cast<size_t>(M) * 3 * H, st))) return rc;
     if ((rc = transpose_bf16<2>(s.dA, 3 * H, M, 3 * H, s.Gt, Mp, st))) return rc;
@@ -1242,15 +1262,27 @@ bool weights_complete(const ance_encoder_config& c, const ance_encoder_weights* 
   return !c.has_head || (ok(w->head_w) && ok(w->head_b) && ok(w->head_ln_g) && ok(w->head_ln_b));
 }
 
+// The sequence lengths the training calls accept: 8, 16, 32, 64 and 128, and the multiples of 128 up to the handle's
+// train_max_len (ANCE_ERR_UNSUPPORTED above it; ANCE_ERR_INVALID for other lengths up to it).
+int check_train_len(const ance_encoder* e, int L, const char* fn) {
+  if (L > attn::kTile && (L > e->train_max_len || L > 512)) {
+    ance::set_error("%s: L = %d; the backward covers sequences of up to %d tokens on this handle (train_max_len; 128, 256, 384 "
+                    "or 512)", fn, L, e->train_max_len);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  ANCE_REQUIRE((L > attn::kTile && L % attn::kTile == 0) || (L <= attn::kTile && attn::kTile % L == 0 && L >= 8),
+               "%s: L = %d unsupported (need 8, 16, 32, 64, 128 or a multiple of 128 up to train_max_len %d)", fn, L,
+               e->train_max_len);
+  return ANCE_OK;
+}
+
 }  // namespace
 
 extern "C" int ance_encoder_train_workspace(ance_encoder_t e, int B, int L, size_t* bytes) {
   ANCE_REQUIRE(e != nullptr && bytes != nullptr, "ance_encoder_train_workspace: null argument");
   ANCE_REQUIRE(B > 0 && L > 0, "ance_encoder_train_workspace: empty batch");
-  if (L > attn::kTile) {
-    ance::set_error("ance_encoder_train_workspace: L = %d; the backward covers sequences of up to 128 tokens", L);
-    return ANCE_ERR_UNSUPPORTED;
-  }
+  if (L > attn::kTile)
+    if (const int rc = check_train_len(e, L, "ance_encoder_train_workspace")) return rc;
   *bytes = train_layout(e->cfg, B, L).total;
   return ANCE_OK;
 }
@@ -1261,11 +1293,7 @@ extern "C" int ance_encoder_forward_train(ance_encoder_t e, const int32_t* ids_d
   ANCE_REQUIRE(ids_dev && out_dev && ws_dev, "ance_encoder_forward_train: null buffer");
   ANCE_REQUIRE((lens_dev != nullptr) != (mask_dev != nullptr), "ance_encoder_forward_train: pass exactly one of lens_dev / mask_dev");
   ANCE_REQUIRE(B > 0 && L > 0, "ance_encoder_forward_train: empty batch");
-  if (L > attn::kTile) {
-    ance::set_error("ance_encoder_forward_train: L = %d; the backward covers sequences of up to 128 tokens", L);
-    return ANCE_ERR_UNSUPPORTED;
-  }
-  ANCE_REQUIRE(128 % L == 0 && L >= 8, "ance_encoder_forward_train: L = %d unsupported (need a divisor of 128, >= 8)", L);
+  if (const int rc = check_train_len(e, L, "ance_encoder_forward_train")) return rc;
   ANCE_REQUIRE((reinterpret_cast<uintptr_t>(ws_dev) & 255u) == 0, "ance_encoder_forward_train: the workspace must be 256-byte aligned");
   const ance_encoder_config& c = e->cfg;
   ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "ance_encoder_forward_train: L = %d exceeds max_position_embeddings %d", L, c.max_pos);
@@ -1526,6 +1554,10 @@ extern "C" int ance_encoder_set_param(ance_encoder_t e, const char* name, double
     ANCE_REQUIRE(value == 1 || value == 16, "varlen_align must be 1 or 16");
     e->varlen_align = static_cast<int>(value);
   }
+  else if (!strcmp(name, "train_max_len")) {
+    ANCE_REQUIRE(value == 128 || value == 256 || value == 384 || value == 512, "train_max_len must be 128, 256, 384 or 512");
+    e->train_max_len = static_cast<int>(value);
+  }
   else { ance::set_error("ance_encoder_set_param: unknown parameter '%s'", name); return ANCE_ERR_INVALID; }
   return ANCE_OK;
 }
@@ -1595,7 +1627,9 @@ extern "C" int ance_encoder_debug_grads(ance_encoder_t e, int slot, float* out_d
 
 extern "C" int ance_dbg_train_layout(ance_encoder_t e, int B, int L, size_t* out) {
   ANCE_REQUIRE(e != nullptr && out != nullptr, "ance_dbg_train_layout: null argument");
-  ANCE_REQUIRE(B > 0 && L > 0 && L <= attn::kTile, "ance_dbg_train_layout: need B > 0 and 0 < L <= 128 (B = %d, L = %d)", B, L);
+  ANCE_REQUIRE(B > 0 && L > 0 && (L <= attn::kTile || (L % attn::kTile == 0 && L <= e->train_max_len)),
+               "ance_dbg_train_layout: need B > 0 and 0 < L <= 128, or L a multiple of 128 up to the handle's train_max_len %d "
+               "(B = %d, L = %d)", e->train_max_len, B, L);
   const TrainLayout t = train_layout(e->cfg, B, L);
   const size_t f[kTrainLayoutFields] = {t.ids, t.kbias, t.layers, t.per_layer, t.x_in, t.qkv, t.ctx, t.t1,
                                         t.x1, t.u, t.ff, t.t2, t.x_final, t.head_in, t.total};
@@ -1702,6 +1736,27 @@ extern "C" int ance_dbg_attention_backward(int fmt, const void* qkv_dev, const f
   return attn_bwd<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st);
 }
 
+extern "C" int ance_dbg_attention_backward_long(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                                int cls_only, int B, int L, int heads, float* dqkv_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_attention_backward_long: unknown operand format %d", fmt);
+  ANCE_REQUIRE(qkv_dev && kbias_dev && dout_bf16_dev && dqkv_dev, "ance_dbg_attention_backward_long: null buffer");
+  ANCE_REQUIRE(aligned16(qkv_dev) && aligned16(dout_bf16_dev) && aligned16(dqkv_dev),
+               "ance_dbg_attention_backward_long: qkv, dout and dqkv must be 16-byte aligned");
+  ANCE_REQUIRE(heads >= 1 && heads <= 16, "ance_dbg_attention_backward_long: heads = %d outside [1, 16]", heads);
+  ANCE_REQUIRE(B > 0 && (L == 256 || L == 384 || L == 512), "ance_dbg_attention_backward_long: need B > 0 and L in {256, 384, 512} (B = %d, L = %d)", B, L);
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* qkv = reinterpret_cast<const uint16_t*>(qkv_dev);
+  const auto* dout = reinterpret_cast<const uint16_t*>(dout_bf16_dev);
+  float* stats = nullptr;
+  ANCE_CUDA(cudaMallocAsync(&stats, bwdl::stats_floats(B, L, heads) * 4, st));
+  const int rc = (fmt == ANCE_FMT_BF16)
+                     ? attn_bwd_long<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st)
+                     : attn_bwd_long<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st);
+  ANCE_CUDA(cudaFreeAsync(stats, st));
+  return rc;
+}
+
 extern "C" int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
                                             const float* gamma_dev, float eps, const float* dy_dev, float* dx_dev,
                                             float* dgamma_dev, float* dbeta_dev, float* dsum_dev, void* stream) {
@@ -1741,8 +1796,8 @@ extern "C" int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L,
                                            void* stream) {
   ANCE_REQUIRE(ids_dev && word_dev && pos_dev && type_dev && dE_dev && E_dev && dword_dev && dpos_dev,
                "ance_dbg_embedding_backward: null buffer");
-  ANCE_REQUIRE(B > 0 && L > 0 && L <= attn::kTile && H > 0 && vocab > 0 && max_pos > 0,
-               "ance_dbg_embedding_backward: need B, H, vocab, max_pos > 0 and 0 < L <= 128 (B = %d, L = %d)", B, L);
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= bwd::kEmbedMaxL && H > 0 && vocab > 0 && max_pos > 0,
+               "ance_dbg_embedding_backward: need B, H, vocab, max_pos > 0 and 0 < L <= 512 (B = %d, L = %d)", B, L);
   if (const int rc = require_sm90(nullptr)) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int M = B * L;

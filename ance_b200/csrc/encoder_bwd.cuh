@@ -1,4 +1,5 @@
-// encoder_bwd.cuh — kernels of the encoder's backward pass (sequences of up to 128 tokens), included by encoder.cu.
+// encoder_bwd.cuh — kernels of the encoder's backward pass, included by encoder.cu (the attention backward of sequences
+// longer than 128 tokens is attn_bwd_long.cuh).
 //
 // The backward GEMMs (dgrad dX = dY W, wgrad dW = dY^T X) run on the forward's own wgmma mainloop and EpStore epilogue
 // (encoder.cu: linear<kFmtBF16>) over transposed bf16 copies made here; everything else is in this file:
@@ -376,26 +377,32 @@ __global__ void add_rows_kernel(float* __restrict__ dst, size_t dst_row_stride, 
 
 // The embedding LayerNorm's input E = (word[id] + pos[p]) + type[0] (fp32, the forward's association) and the position id
 // of every token of sequence b = blockIdx.x; positions follow the forward's rule (RoBERTa: cumsum of non-pad tokens + pad,
-// pad tokens at pad; BERT: 0 .. L-1).  Ids / positions out of range are clamped as in the forward.
+// pad tokens at pad; BERT: 0 .. L-1).  Ids / positions out of range are clamped as in the forward.  L <= kEmbedMaxL: the
+// scan runs over chunks of 256 tokens, carrying the count of the chunks before.
+constexpr int kEmbedMaxL = 512;
 __global__ void __launch_bounds__(256) embed_sum_kernel(const int32_t* __restrict__ ids_all, int L, int H, int roberta,
                                                         int pad_id, int vocab, int max_pos, const float* __restrict__ word,
                                                         const float* __restrict__ pos, const float* __restrict__ type,
                                                         float* __restrict__ E, int32_t* __restrict__ pos_out) {
-  __shared__ int s_pos[128];
+  __shared__ int s_pos[kEmbedMaxL];
   __shared__ int s_warp_cnt[8];
   const int b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int32_t* ids = ids_all + static_cast<size_t>(b) * L;
-  {
-    const int t = threadIdx.x;
+  for (int base = 0, carry = 0; base < L; base += 256) {
+    const int t = base + threadIdx.x;
     const int flag = (t < L && ids[t] != pad_id) ? 1 : 0;
     const unsigned bal = __ballot_sync(0xffffffffu, flag);
     if (lane == 0) s_warp_cnt[warp] = __popc(bal);
     __syncthreads();
-    int pre = 0;
-    for (int w2 = 0; w2 < warp; ++w2) pre += s_warp_cnt[w2];
+    int pre = carry, total = carry;
+    for (int w2 = 0; w2 < 8; ++w2) {
+      if (w2 < warp) pre += s_warp_cnt[w2];
+      total += s_warp_cnt[w2];
+    }
     const int incl = pre + __popc(bal & ((2u << lane) - 1u));
     if (t < L) s_pos[t] = roberta ? (flag ? incl + pad_id : pad_id) : t;
+    carry = total;
     __syncthreads();
   }
   for (int t = warp; t < L; t += 8) {

@@ -11,7 +11,8 @@ The classes are ``nn.Module``s whose parameters carry the checkpoint's own key n
 so ``load_state_dict`` / ``.to(device)`` / DDP wrapping behave as with the reference; the forward
 is NOT PyTorch: ``query_emb`` / ``body_emb`` run the hand-written sm_90a encoder of
 libance_b200.so (csrc/encoder.cu).  There is no CPU path — calling them with CPU tensors raises.
-Training: after ``model.set_trainable(True)`` (rdot_nll, inputs of up to 128 tokens) ``query_emb`` / ``body_emb`` /
+Training: after ``model.set_trainable(True)`` (inputs of up to 128 tokens) or ``model.set_trainable(True, max_len=512)``
+(up to 512: FirstP documents, MaxP chunks; DPR's BiEncoder needs ``max_len=256``) ``query_emb`` / ``body_emb`` /
 ``forward()`` build an autograd graph whose backward runs the encoder's own backward kernels, so ``loss.backward()``
 fills the parameters' ``.grad``; by default the outputs carry no graph.
 """
@@ -231,7 +232,8 @@ class _CudaEncoder:
         return True
 
     def forward_train(self, ids: torch.Tensor, lens: Optional[torch.Tensor], mask: Optional[torch.Tensor]):
-        """forward() of a whole [B, L <= 128] batch that also keeps what the backward needs.  -> (out fp32 [B, H],
+        """forward() of a whole [B, L] batch (L <= 128, or a multiple of 128 up to the handle's train_max_len) that also
+        keeps what the backward needs.  -> (out fp32 [B, H],
         workspace tensor for backward())."""
         B, L = ids.shape
         n = C.c_size_t()
@@ -325,14 +327,19 @@ class _B200Encoder(nn.Module):
     #: Same tensor-core rate either way.
     encoder_operand = os.environ.get("ANCE_B200_ENCODER_OPERAND", "fp16")
 
-    #: set_trainable(True): embeddings computed while grad is enabled carry an autograd graph (dense, L <= 128)
+    #: set_trainable(True): embeddings computed while grad is enabled carry an autograd graph (dense, L <= _train_max_len)
     _trainable = False
+    _train_max_len = 128
 
-    def set_trainable(self, on: bool = True):
+    def set_trainable(self, on: bool = True, max_len: int = 128):
         """Opt in to gradients: while torch grad mode is on, query_emb / body_emb / encode_lens (dense batches of up to
-        128 tokens) and the triplet forward() return tensors whose backward runs the encoder's backward kernels; the
-        other encode paths raise instead of returning detached results.  Off by default."""
+        `max_len` tokens per sequence or MaxP chunk: 8, 16, 32, 64 or 128, or a multiple of 128 up to max_len) and the
+        triplet forward() return tensors whose backward runs the encoder's backward kernels; the other encode paths raise
+        instead of returning detached results.  max_len is 128, 256, 384 or 512.  Off by default."""
+        if max_len not in (128, 256, 384, 512):
+            raise ValueError(f"max_len must be 128, 256, 384 or 512, got {max_len!r}")
         self._trainable = bool(on)
+        self._train_max_len = int(max_len)
         return self
 
     def _grad_path(self) -> bool:
@@ -340,20 +347,29 @@ class _B200Encoder(nn.Module):
 
     def _refuse_grad(self, what: str) -> None:
         if self._grad_path():
-            raise _lib.AnceError(f"{what} has no backward: trainable encoders take dense batches of up to 128 tokens "
-                                 "through query_emb / body_emb / encode_lens (or run this under torch.no_grad())")
+            raise _lib.AnceError(f"{what} has no backward: trainable encoders take dense batches of up to max_len = "
+                                 f"{self._train_max_len} tokens through query_emb / body_emb / encode_lens (or run this "
+                                 "under torch.no_grad())")
 
     def _train_emb(self, enc, backbone, head, ids, lens, mask):
         B, L = ids.shape
-        if L > 128:
-            raise _lib.AnceError(f"inputs of {L} tokens have no backward: the trainable encoder covers up to 128 tokens "
-                                 "(run longer inputs under torch.no_grad())")
+        max_len = self._train_max_len
+        if L > max_len:
+            raise _lib.AnceError(f"inputs of {L} tokens have no backward: the trainable encoder covers up to max_len = "
+                                 f"{max_len} tokens (set_trainable(True, max_len=...) takes 128, 256, 384 or 512; or run "
+                                 "longer inputs under torch.no_grad())")
+        if L > 128 and L % 128:
+            raise _lib.AnceError(f"inputs of {L} tokens have no backward: above 128 tokens the trainable encoder takes "
+                                 "multiples of 128 (pad the batch to 256, 384 or 512)")
         if B * L > enc.max_tokens:
             raise _lib.AnceError(f"a trainable batch of {B} x {L} tokens exceeds max_tokens {enc.max_tokens}")
         # The device weights are refreshed from the parameters before every training forward, whatever their `_version`
         # says: optimizers that write through `p.data` (the reference trainer's Lamb, transformers' AdamW) do not bump it.
         if not enc.update_weights(backbone, head):
             raise _lib.AnceError("a trainable encoder needs contiguous fp32 parameters on the inputs' device")
+        if getattr(enc, "_train_max_len", 128) != max_len:
+            enc.set_param("train_max_len", max_len)
+            enc._train_max_len = max_len
         embs, layers, hd = _param_groups(backbone, head)
         params = embs + [t for l in layers for t in l] + hd
         return _TrainableEncode.apply(enc, len(layers), ids, lens, mask, *params)
@@ -397,7 +413,7 @@ class _B200Encoder(nn.Module):
     # -- reference `NLL.forward` (model/models.py:58-84) ------------------------------------------------------
     # Same signature and return values as the reference: embeddings when only one side is given, `(loss,)` for a
     # (query, positive, negative) triplet batch.  After set_trainable(True), with grad enabled, the loss carries an
-    # autograd graph through the encoder's backward kernels (inputs of up to 128 tokens); otherwise it is computed
+    # autograd graph through the encoder's backward kernels (inputs of up to max_len tokens); otherwise it is computed
     # under no_grad, as the value the trainer logs.
     @staticmethod
     def _pair_logits(q_embs, x_embs, input_ids_x, attention_mask_x):
@@ -550,7 +566,9 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
         self.base_len = 512
 
     def body_emb(self, input_ids, attention_mask):
-        self._refuse_grad("the multi-chunk body_emb")
+        """[B, chunks * 512] -> [B, chunks, 768]; trainable (every chunk through the dense backward) with max_len >= 512."""
+        if self._train_max_len < self.base_len:
+            self._refuse_grad("the multi-chunk body_emb (its 512-token chunks need set_trainable(True, max_len=512))")
         batchS, full_length = input_ids.shape
         chunk_factor = full_length // self.base_len
         if chunk_factor == 0 or full_length % chunk_factor != 0:
@@ -558,7 +576,10 @@ class RobertaDot_CLF_ANN_NLL_MultiChunk(RobertaDot_NLL_LN):
         seq = full_length // chunk_factor
         ids, mask = self._prep(input_ids.reshape(batchS * chunk_factor, seq),
                                attention_mask.reshape(batchS * chunk_factor, seq))
-        emb = self._encoder(ids.device).forward(ids, None, mask)
+        if self._grad_path():
+            emb = self._train_emb(self._encoder(ids.device), self.roberta, (self.embeddingHead, self.norm), ids, None, mask)
+        else:
+            emb = self._encoder(ids.device).forward(ids, None, mask)
         return emb.reshape(batchS, chunk_factor, emb.shape[-1])
 
     def _pair_logits(self, q_embs, x_embs, input_ids_x, attention_mask_x):
@@ -654,10 +675,13 @@ class BiEncoder(_B200Encoder):
         self.ctx_model = _backbone(d.vocab_size, d.hidden_size, d.num_hidden_layers, d.intermediate_size,
                                    d.max_position_embeddings, d.type_vocab_size, d.pad_token_id, d.layer_norm_eps)
 
-    def set_trainable(self, on: bool = True):
-        if on:
-            raise NotImplementedError("the DPR BiEncoder has no backward in ance_b200 (rdot_nll only)")
-        return super().set_trainable(False)
+    def set_trainable(self, on: bool = True, max_len: Optional[int] = None):
+        """As _B200Encoder.set_trainable for both BERT encoders; training needs an explicit max_len (DPR's inputs are 256
+        tokens: set_trainable(True, max_len=256))."""
+        if on and max_len is None:
+            raise NotImplementedError("the DPR BiEncoder trains on 256-token inputs: call set_trainable(True, max_len=256) "
+                                      "(or 128 / 384 / 512 for other input lengths)")
+        return super().set_trainable(on, 128 if max_len is None else max_len)
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         # HF BertModel checkpoints carry pooler.* and position_ids buffers the path never uses
@@ -671,6 +695,8 @@ class BiEncoder(_B200Encoder):
     def _emb(self, name, backbone, input_ids, attention_mask):
         ids, mask = self._prep(input_ids, attention_mask)
         enc = self._enc_for(name, backbone, _lib.ANCE_ARCH_BERT, self.dims.num_attention_heads, 0, None, ids.device)
+        if self._grad_path():
+            return self._train_emb(enc, backbone, None, ids, None, mask)
         return enc.forward(ids, None, mask)
 
     def query_emb(self, input_ids, attention_mask):
@@ -683,6 +709,7 @@ class BiEncoder(_B200Encoder):
         """Same result as _emb(..., input_ids != 0) (DPR_data.py:283 mask) at the cost of the real tokens: rows whose
         nonzero ids form a non-empty prefix go through the packed forward, the others through the dense one.  The lengths
         are read from `ids_host` (the host copy of input_ids; copied back when not given)."""
+        self._refuse_grad("query_emb_packed / body_emb_packed")
         if input_ids.device.type != "cuda":
             raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
         ids = input_ids.to(torch.int32).contiguous()
@@ -712,10 +739,16 @@ class BiEncoder(_B200Encoder):
         """body_emb(input_ids, input_ids != 0) computing the real tokens only (align: see encode_lens_packed)."""
         return self._emb_packed("ctx", self.ctx_model, input_ids, align, ids_host)
 
-    @torch.no_grad()
     def forward(self, query_ids, attention_mask_q, input_ids_a=None, attention_mask_a=None, input_ids_b=None,
                 attention_mask_b=None):
-        """model/models.py:253-266 (evaluation only, no autograd): (q, a) embeddings, or `(loss,)` for triplets."""
+        """model/models.py:253-266: (q, a) embeddings (the in-batch-negative form), or `(loss,)` for triplets.  Both carry
+        an autograd graph after set_trainable(True, max_len=...) with grad enabled; otherwise they are computed under
+        no_grad."""
+        with contextlib.nullcontext() if self._grad_path() else torch.no_grad():
+            return self._bi_forward(query_ids, attention_mask_q, input_ids_a, attention_mask_a, input_ids_b,
+                                    attention_mask_b)
+
+    def _bi_forward(self, query_ids, attention_mask_q, input_ids_a, attention_mask_a, input_ids_b, attention_mask_b):
         q_embs = self.query_emb(query_ids, attention_mask_q)
         a_embs = self.body_emb(input_ids_a, attention_mask_a)
         if input_ids_b is None:

@@ -210,7 +210,9 @@ int ance_encoder_forward_packed(ance_encoder_t enc, const int32_t* ids_dev, cons
  * downstream, so out-projection / FFN / LayerNorm run on those rows only (result-identical; bench.py reports
  * the executed FLOPs beside the algorithmic ones).  "ln_rows_per_warp" (1, 2, 4, or 3 = two rows held packed; default 2, process-wide): rows a warp
  * of the LayerNorm kernel normalises side by side (bit-identical results; default 2).  "varlen_align" (1 | 16):
- * see ance_encoder_forward_varlen and ance_encoder_forward_packed. */
+ * see ance_encoder_forward_varlen and ance_encoder_forward_packed.  "train_max_len" (128, 256, 384 or 512; default 128,
+ * per handle): the longest sequence ance_encoder_train_workspace, ance_encoder_forward_train and ance_dbg_train_layout
+ * accept; above 128 they take the multiples of 128 up to it (the attention backward of L > 128 is a key-blocked kernel). */
 int ance_encoder_set_param(ance_encoder_t enc, const char* name, double value);
 /* Input / output validation, deferred so that forward stays asynchronous: synchronises `stream` and returns
  * ANCE_ERR_INVALID if any forward since the last check saw a token id outside [0, vocab_size) or a position
@@ -224,8 +226,8 @@ int ance_encoder_check(ance_encoder_t enc, void* stream);
 int ance_encoder_debug_hidden(ance_encoder_t enc, int layer, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Training: gradients of the dense forward for sequences of up to 128 tokens (the trainer side of
- * model/models.py:58-84, NLL.forward -> loss.backward()).
+ * Training: gradients of the dense forward for sequences of up to 128 tokens, or up to 512 on a handle whose
+ * "train_max_len" allows it (the trainer side of model/models.py:58-84, NLL.forward -> loss.backward()).
  * ------------------------------------------------------------------------------------------------ */
 /* Gradient buffers: the layout of ance_encoder_weights / ance_layer_weights with DEVICE fp32 pointers (16-byte aligned),
  * every one required (the head's only with has_head).  ance_encoder_backward OVERWRITES them. */
@@ -243,11 +245,13 @@ typedef struct {
 } ance_encoder_grads;
 
 /* Bytes of device workspace one ance_encoder_forward_train of a [B, L] batch keeps for its backward (about
- * 16 hidden + 4 ffn bytes per token and layer: 24.6 KB at hidden 768, ffn 3072).  ANCE_ERR_UNSUPPORTED for L > 128. */
+ * 16 hidden + 4 ffn bytes per token and layer: 24.6 KB at hidden 768, ffn 3072).  ANCE_ERR_UNSUPPORTED for L > 128 unless
+ * L is a multiple of 128 up to the handle's "train_max_len" (ANCE_ERR_UNSUPPORTED above it). */
 int ance_encoder_train_workspace(ance_encoder_t enc, int B, int L, size_t* bytes);
 /* ance_encoder_forward with every activation the backward needs saved in ws_dev (256-byte aligned, the size above; one
  * workspace per forward whose backward is still to come; each forward_train is followed by at most one backward).  out_dev is bit-identical to ance_encoder_forward's.
- * L must be 8, 16, 32, 64 or 128 (ANCE_ERR_UNSUPPORTED above 128) and B * L <= max_tokens. */
+ * L must be 8, 16, 32, 64 or 128, or a multiple of 128 up to "train_max_len" (ANCE_ERR_UNSUPPORTED above it), and
+ * B * L <= max_tokens. */
 int ance_encoder_forward_train(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev,
                                int B, int L, void* ws_dev, float* out_dev, void* stream);
 /* Gradients of sum(d_out o out) with respect to every weight, for the forward that filled ws_dev (the weights must not
@@ -329,6 +333,11 @@ int ance_dbg_layer_norm(int fmt, const void* in_dev, int in_f32, int64_t in_ld, 
  * -> dqkv [B * L, 3 * 64 heads] fp32. */
 int ance_dbg_attention_backward(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
                                 int cls_only, int B, int L, int heads, float* dqkv_dev, void* stream);
+/* The backward's attention kernels for L in {256, 384, 512} (the launch ance_encoder_backward makes there): the arguments
+ * of ance_dbg_attention_backward, qkv, dout and dqkv 16-byte aligned.  Key-blocked on the tensor cores: a query-block
+ * kernel writes dQ and per-row softmax statistics (scratch allocated per call), a key-block kernel then dK and dV. */
+int ance_dbg_attention_backward_long(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                     int cls_only, int B, int L, int heads, float* dqkv_dev, void* stream);
 /* The backward's LayerNorm kernel: input rows as for ance_dbg_layer_norm, dy / dx fp32 [rows, H]; dgamma, dbeta and dsum
  * (column sum of dx) [H] may each be null. */
 int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
@@ -338,7 +347,7 @@ int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_
 int ance_dbg_gelu_backward(int fmt, const void* u_dev, float* g_dev, int64_t n, void* stream);
 /* The backward's embedding kernels: E [B * L, H] fp32 = (word[id] + pos[p]) + type[0], the LayerNorm input the backward
  * recomputes (positions by the arch's rule, roberta = 1 for RoBERTa's), then dword [vocab, H] and dpos [max_pos, H] are
- * zeroed and the rows of dE [B * L, H] scatter-added into them (no gradient for the padding_idx rows).  L <= 128. */
+ * zeroed and the rows of dE [B * L, H] scatter-added into them (no gradient for the padding_idx rows).  L <= 512. */
 int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int roberta, int pad_id, int vocab, int max_pos,
                                 const float* word_dev, const float* pos_dev, const float* type_dev, const float* dE_dev,
                                 float* E_dev, float* dword_dev, float* dpos_dev, void* stream);
@@ -346,7 +355,8 @@ int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int
  * columns R .. dst_ld - 1 of dst set to zero. */
 int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, int R, int C, void* dst_dev, int64_t dst_ld,
                             void* stream);
-/* Host-only: the byte offsets of the workspace ance_encoder_forward_train fills for a [B, L <= 128] batch, out[15] =
+/* Host-only: the byte offsets of the workspace ance_encoder_forward_train fills for a [B, L] batch (L <= 128, or a multiple
+ * of 128 up to the handle's "train_max_len"), out[15] =
  * ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total.  ids [B * L] int32 and kbias
  * [B * L] fp32 (log2 units) sit at their offsets; layer l's slots at layers + l * per_layer + (x_in .. t2); x_final
  * [B, hidden] 16-bit (the last layer's CLS outputs) and head_in [B, hidden] fp32 (the head LayerNorm's input) at theirs.
