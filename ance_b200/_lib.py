@@ -106,6 +106,9 @@ SIGNATURES = {
     "ance_encoder_train_workspace": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "ance_encoder_forward_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ance_encoder_forward_train_dropout": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                     C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_uint64,
+                                                     C.c_void_p]),
     "ance_encoder_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(EncoderGrads), C.c_void_p]),
     "ance_encoder_update_weights": (C.c_int, [C.c_void_p, C.POINTER(EncoderWeights), C.c_void_p]),
     "ance_encoder_debug_grads": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -132,6 +135,10 @@ SIGNATURES = {
                                                C.c_void_p]),
     "ance_dbg_gelu_backward": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "ance_dbg_embedding_backward": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p] * 8),
+    "ance_dbg_attention_backward_dropout": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                      C.c_int, C.c_int, C.c_float, C.c_uint64, C.c_int, C.c_void_p,
+                                                      C.c_void_p]),
+    "ance_dbg_dropout_bits": (C.c_int, [C.c_uint64, C.c_uint64, C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p]),
     "ance_dbg_transpose_bf16": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p]),
     "ance_dbg_train_layout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),

@@ -28,6 +28,7 @@
 // block 0.
 #pragma once
 #include "act16.cuh"
+#include "dropout.cuh"
 #include "tc05.cuh"
 
 namespace attn {
@@ -57,6 +58,9 @@ struct Params {
   const int32_t* row_hi;
   // attention_multi_kernel<kPacked = true>: per 128-row tile, (first key row, number of 128-key blocks) of its work items
   const int2* tile_kv;
+  // kDrop kernels (dense sequences only, row_lo null): dropout of the probabilities, site 1 (dropout.cuh).  The dropped
+  // entries of the 16-bit P are zero, the row sum l keeps every p, and ctx = O * (drop.scale / l).
+  drop::Cfg drop;
 };
 
 struct Smem {
@@ -87,7 +91,7 @@ constexpr int kThreads = 256;   // attention_multi_kernel: warp 0 TMA, 1-3 idle,
 // arithmetic); producer and warpgroup derive the block order from the same loop nest.
 // kPacked: a variable-length row plan (p.row_lo, p.tile_kv) of sequences longer than 128 tokens.
 // FMT: 16-bit format of Q / K / V, of the probabilities P and of the output (act16.cuh).
-template <bool kPacked, uint32_t FMT>
+template <bool kPacked, uint32_t FMT, bool kDrop = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -200,6 +204,9 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
       // end of the whole 32-key chunks of the own sequence (counted from its first key): the keys the dense kernel,
       // with the sequence at key 0, handles in unmasked chunks
       const int seq_full = seq_lo + ((seq_hi - seq_lo) & ~31);
+      // kDrop (dense, L >= 256): this row is query qi of sequence tok / L; its keys are the item's kv0 .. kv0 + L - 1
+      const uint32_t d_qi = kDrop ? static_cast<uint32_t>((tok0 + row) % p.L) : 0u;
+      const uint32_t d_c2 = kDrop ? static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h) : 0u;
       float m_run = -INFINITY, l_run = 0.f;
       float o[kDh];
 #pragma unroll
@@ -288,6 +295,22 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
             } else {
               uint32_t v[32];
               acc_ld_x32(srow + c, v);
+              uint4 dw[4];   // kDrop: the four calls of this 32-key chunk (dw[q] covers the key pairs q, q + 4, q + 8, q + 12)
+              if constexpr (kDrop) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q)
+                  dw[q] = drop::philox(p.drop.k0, p.drop.k1, 4u * static_cast<uint32_t>((j * kTile + c) >> 5) + q, d_qi, d_c2,
+                                       p.drop.stream);
+              }
+              // zero the dropped entries of the 16-bit P (after the row sum, which keeps them)
+              auto dropped = [&](int k, uint32_t& pp) {
+                if constexpr (kDrop) {
+                  const uint32_t wq = drop::word(dw[(k >> 1) & 3], (k >> 3) & 3);
+                  const uint32_t lo = drop::keep(wq, 0, p.drop.thr) ? 0x0000FFFFu : 0u;
+                  const uint32_t hi = drop::keep(wq, 1, p.drop.thr) ? 0xFFFF0000u : 0u;
+                  pp &= lo | hi;
+                }
+              };
               if (sc_ == 1) {
 #pragma unroll
                 for (int i = 0; i < 32; i += 2) {
@@ -297,6 +320,7 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
                   const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
                   rs_ += p0 + p1;
                   pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
+                  dropped(i, pk[i >> 1]);
                 }
               } else {
 #pragma unroll
@@ -312,6 +336,7 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
                   const float p0 = ex2_ftz(u0), p1 = ex2_ftz(u1);
                   rs_ += p0 + p1;
                   pk[i >> 1] = act16::Act<FMT>::pack2(p0, p1);
+                  dropped(i, pk[i >> 1]);
                 }
               }
             }
@@ -418,7 +443,7 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
       }
       // ctx tile = o / l in 16 bits: staged in this group's P buffer (the PV MMA has finished reading it), one TMA store
       {
-        const float inv = 1.0f / l_run;
+        const float inv = kDrop ? p.drop.scale / l_run : 1.0f / l_run;
 #pragma unroll
         for (int c = 0; c < kDh; c += 32) {
           uint32_t pk[16];
@@ -481,11 +506,34 @@ struct RowSt {
   bool plain;
 };
 
+// kDrop: a row's dropout counter words: query index qi in its sequence, c2 = sequence * heads + head, and lo, the tile
+// column of the sequence's key 0
+struct DropRow {
+  uint32_t qi, c2;
+  int lo;
+};
+
+// the dropout call of 32-key chunk cc (tile columns 32 cc ..) of a row, as the lane with q4 uses it: word m covers the
+// columns 32 cc + 8 m + 2 q4 + {0, 1}.  A sequence shorter than 32 keys (L = 8, 16) lies in one call whose words are
+// rotated by the sequence's offset inside its 32-key chunk; the columns of other sequences get words that are not theirs,
+// where p is exactly 0.
+__device__ __forceinline__ uint4 drop_bits(const drop::Cfg& dc, const DropRow& r, int L, int cc, int q4) {
+  if (L < 32) {
+    const uint4 w = drop::philox(dc.k0, dc.k1, static_cast<uint32_t>(q4), r.qi, r.c2, dc.stream);
+    const int rot = (r.lo >> 3) & 3;
+    return rot == 0 ? w : rot == 1 ? make_uint4(w.w, w.x, w.y, w.z) : rot == 2 ? make_uint4(w.z, w.w, w.x, w.y)
+                                                                                : make_uint4(w.y, w.z, w.w, w.x);
+  }
+  return drop::philox(dc.k0, dc.k1, 4u * static_cast<uint32_t>((32 * cc - r.lo) >> 5) + q4, r.qi, r.c2, dc.stream);
+}
+
 // Softmax of the two rows (r, r + 8) held by accumulator `d` (m64n128 fragment): P packed in pairs into `pk` (the A
 // fragments of the 8 k steps of P V), row sums (reduced over the quad) into rsum.
-template <bool kPacked, uint32_t FMT>
+template <bool kPacked, uint32_t FMT, bool kDrop = false>
 __device__ __forceinline__ void softmax_pair(float (&d)[64], const RowSt& ra, const RowSt& rb, const float* sbias, int q4,
-                                             float scale_log2, uint32_t (&pk)[32], float& la, float& lb) {
+                                             float scale_log2, uint32_t (&pk)[32], float& la, float& lb,
+                                             const Params* dp = nullptr, const DropRow* da = nullptr,
+                                             const DropRow* db = nullptr) {
   const RowSt rs[2] = {ra, rb};
   float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -516,9 +564,16 @@ __device__ __forceinline__ void softmax_pair(float (&d)[64], const RowSt& ra, co
     nm[i] = -m;
   }
   float acc[2] = {0.f, 0.f};
+  uint4 dw[2];   // kDrop: the dropout call of the current 32-key chunk, rows r and r + 8
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int c = j >> 2;
+    if constexpr (kDrop) {
+      if ((j & 3) == 0) {
+        dw[0] = drop_bits(dp->drop, *da, dp->L, c, q4);
+        dw[1] = drop_bits(dp->drop, *db, dp->L, c, q4);
+      }
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {   // h: row r (d[4j], d[4j + 1]) or r + 8 (d[4j + 2], d[4j + 3])
       const bool zero = ((rs[h].st >> (2 * c)) & 3) == 0;
@@ -526,6 +581,10 @@ __device__ __forceinline__ void softmax_pair(float (&d)[64], const RowSt& ra, co
       const float p1 = zero ? 0.f : ex2_ftz(fmaf(d[4 * j + 2 * h + 1], sc[h], nm[h]));
       acc[h] += p0 + p1;
       pk[2 * j + h] = act16::Act<FMT>::pack2(p0, p1);
+      if constexpr (kDrop) {   // the dropped entries of P become 0; the row sum keeps them
+        const uint32_t wq = drop::word(dw[h], j & 3);
+        pk[2 * j + h] &= (drop::keep(wq, 0, dp->drop.thr) ? 0x0000FFFFu : 0u) | (drop::keep(wq, 1, dp->drop.thr) ? 0xFFFF0000u : 0u);
+      }
     }
   }
 #pragma unroll
@@ -537,7 +596,7 @@ __device__ __forceinline__ void softmax_pair(float (&d)[64], const RowSt& ra, co
   lb = acc[1];
 }
 
-template <bool kPacked, uint32_t FMT>
+template <bool kPacked, uint32_t FMT, bool kDrop = false>
 __global__ void __launch_bounds__(kSingleThreads, 1)
 attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmCTX, const Params p) {
   using S = SmemSingle;
@@ -624,9 +683,15 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
     // row has an unmasked key somewhere: exp2(-10000 log2e + s - m) flushes to zero, as exp(-10000 + s - m) does in the
     // reference's fp32 softmax), 1 = no key masked (no bias term), 2 = general.
     RowSt rs[4];
+    DropRow dr[4];   // kDrop (dense): query index, sequence / head word and own-key offset of each row
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int row = r0 + (i & 1) * 8 + (i >> 1) * 64;
+      if constexpr (kDrop) {
+        dr[i].qi = static_cast<uint32_t>((tok0 + row) % p.L);
+        dr[i].c2 = static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h);
+        dr[i].lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;
+      }
       int lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;   // keys of this row's own sequence
       int hi = (p.L >= kTile) ? kTile : lo + p.L;
       if (varlen) {
@@ -664,7 +729,7 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
     // of half 0 is issued before the S of half 1, and wgmmas issue in program order, so the S of half 1 cannot be
     // hoisted above the softmax of half 0: one half of S, P and O is live at a time, and nothing spills.  (The other
     // consumer warpgroup covers the waits.)
-    auto half = [&](int m0, const RowSt& ra, const RowSt& rb) {
+    auto half = [&](int m0, const RowSt& ra, const RowSt& rb, const DropRow& da, const DropRow& db) {
       uint32_t pk[32];
       float l[2];
       {
@@ -678,7 +743,7 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(s);
-        softmax_pair<kPacked, FMT>(s, ra, rb, sbias, q4, p.scale_log2, pk, l[0], l[1]);
+        softmax_pair<kPacked, FMT, kDrop>(s, ra, rb, sbias, q4, p.scale_log2, pk, l[0], l[1], &p, &da, &db);
       }
       float o[kDh / 2];
 #pragma unroll
@@ -696,7 +761,7 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {   // rows m0 + r0 + 8 hh: o[4 j + 2 hh + 0..1], keys 8 j + 2 (t % 4) + 0..1
         const int row = m0 + r0 + 8 * hh;
-        const float inv = 1.0f / l[hh];
+        const float inv = kDrop ? p.drop.scale / l[hh] : 1.0f / l[hh];
         uint8_t* rowp = sout + row * 128 + q4 * 4;
 #pragma unroll
         for (int j = 0; j < kDh / 8; ++j) {
@@ -705,8 +770,8 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
         }
       }
     };
-    half(0, rs[0], rs[1]);
-    half(64, rs[2], rs[3]);
+    half(0, rs[0], rs[1], dr[0], dr[1]);
+    half(64, rs[2], rs[3], dr[2], dr[3]);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[rq.stage]);   // this warp's last read of the stage
     rq.advance();

@@ -20,6 +20,7 @@
 // in registers as the A operand of the next product (the m16n8k16 C and A fragments share their row / column layout).
 #pragma once
 #include "act16.cuh"
+#include "dropout.cuh"
 
 namespace bwdl {
 
@@ -142,12 +143,34 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// kDrop: the forward dropped the probabilities with the mask m of site 1 and scale s (dropout.cuh).  Both kernels then
+// use dP = m o (dO V^T) s (so D = sum_j P dP) and dkv_kernel P~ = m o P s for dV, the mask regenerated per element.
+// dq_kernel: the masked dP of rows (r, r + 8) of key block kb, in place
+template <uint32_t FMT, bool kDrop>
+__device__ __forceinline__ void drop_dp_rows(float (&dp)[8][4], const drop::Cfg& dc, uint32_t qi0, uint32_t c2, int kb, int t) {
+  if constexpr (kDrop) {
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {   // key chunk 2 kb + half: n = 4 half .. 4 half + 3
+        const uint4 w = drop::philox(dc.k0, dc.k1, 4u * (2 * kb + half) + t, qi0 + 8 * hf, c2, dc.stream);
+#pragma unroll
+        for (int m = 0; m < 4; ++m)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& x = dp[4 * half + m][2 * hf + e];
+            x = drop::keep(drop::word(w, m), e, dc.thr) ? x * dc.scale : 0.f;
+          }
+      }
+  }
+}
+
 // accumulator element (n, e) of lane (g = lane / 4, t = lane % 4) sits at row g + 8 (e / 2), column 8 n + 2 t + e % 2
-template <uint32_t FMT>
+template <uint32_t FMT, bool kDrop = false>
 __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                       const uint16_t* __restrict__ dout, int cls_only,
                                                       float* __restrict__ dqkv, float* __restrict__ stats, int L,
-                                                      int heads, float scale_log2) {
+                                                      int heads, float scale_log2, const drop::Cfg dc) {
   constexpr bool kConv = FMT == tc05::kFmtF16;
   __shared__ alignas(16) uint16_t sQ[kBlk * kPitch], sO[kBlk * kPitch], sK[kBlk * kPitch], sV[kBlk * kPitch];
   __shared__ alignas(16) uint16_t sKb_[kConv ? kBlk * kPitch : 8];
@@ -186,6 +209,7 @@ __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict
     zero(dp);
     mma_abt<FMT>(s, aQ, sK, lane);
     mma_abt<tc05::kFmtBF16>(dp, aO, sV, lane);
+    drop_dp_rows<FMT, kDrop>(dp, dc, qb * kBlk + warp * 16 + g, b * heads + h, kb, t);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int n = 0; n < 8; ++n)
@@ -238,6 +262,7 @@ __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict
     zero(dp);
     mma_abt<FMT>(s, aQ, sK, lane);
     mma_abt<tc05::kFmtBF16>(dp, aO, sV, lane);
+    drop_dp_rows<FMT, kDrop>(dp, dc, qb * kBlk + warp * 16 + g, b * heads + h, kb, t);
 #pragma unroll
     for (int n = 0; n < 8; ++n)
 #pragma unroll
@@ -257,11 +282,11 @@ __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict
       *reinterpret_cast<float2*>(dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t) = make_float2(dq[n][2 * hf], dq[n][2 * hf + 1]);
 }
 
-template <uint32_t FMT>
+template <uint32_t FMT, bool kDrop = false>
 __global__ void __launch_bounds__(kThreads) dkv_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                        const uint16_t* __restrict__ dout, int cls_only,
                                                        float* __restrict__ dqkv, const float* __restrict__ stats, int L,
-                                                       int heads, float scale_log2) {
+                                                       int heads, float scale_log2, const drop::Cfg dc) {
   constexpr bool kConv = FMT == tc05::kFmtF16;
   __shared__ alignas(16) uint16_t sQ[kBlk * kPitch], sO[kBlk * kPitch], sK[kBlk * kPitch], sV[kBlk * kPitch];
   __shared__ alignas(16) uint16_t sQb_[kConv ? kBlk * kPitch : 8];
@@ -297,15 +322,37 @@ __global__ void __launch_bounds__(kThreads) dkv_kernel(const uint16_t* __restric
     zero(dp);
     mma_abt<FMT>(s, aK, sQ, lane);                // S^T: rows = keys, columns = queries
     mma_abt<tc05::kFmtBF16>(dp, aV, sO, lane);    // dP^T
+    if constexpr (kDrop) {
+      // this lane's keys jr, jr + 8 (jr = kb 64 + warp 16 + g) share one call per query (same 32-key chunk and key pair
+      // index); their words are (jr >> 3) & 3 and the next one
+      const int jr = kb * kBlk + warp * 16 + g;
 #pragma unroll
-    for (int n = 0; n < 8; ++n)
+      for (int n = 0; n < 8; ++n)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int i = n * 8 + 2 * t + (e & 1);
-        const float p = exp2f(fmaf(s[n][e], scale_log2, kb_r[e >> 1]) - sM[i]) * sI[i];
-        s[n][e] = p;
-        dp[n][e] = p * (dp[n][e] - sD[i]) * 0.125f;
-      }
+        for (int eq = 0; eq < 2; ++eq) {
+          const uint4 w = drop::philox(dc.k0, dc.k1, 4u * (jr >> 5) + ((jr >> 1) & 3), qb * kBlk + n * 8 + 2 * t + eq,
+                                       b * heads + h, dc.stream);
+#pragma unroll
+          for (int hk = 0; hk < 2; ++hk) {
+            const int e = 2 * hk + eq;
+            const int i = n * 8 + 2 * t + eq;
+            const float p = exp2f(fmaf(s[n][e], scale_log2, kb_r[hk]) - sM[i]) * sI[i];
+            const bool kp = drop::keep(drop::word(w, ((jr >> 3) & 3) + hk), jr & 1, dc.thr);
+            s[n][e] = kp ? p * dc.scale : 0.f;
+            dp[n][e] = p * ((kp ? dp[n][e] * dc.scale : 0.f) - sD[i]) * 0.125f;
+          }
+        }
+    } else {
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int i = n * 8 + 2 * t + (e & 1);
+          const float p = exp2f(fmaf(s[n][e], scale_log2, kb_r[e >> 1]) - sM[i]) * sI[i];
+          s[n][e] = p;
+          dp[n][e] = p * (dp[n][e] - sD[i]) * 0.125f;
+        }
+    }
     uint32_t aP[4][4];
     acc_to_a(aP, s);
     mma_ab(dv, aP, sO, lane);

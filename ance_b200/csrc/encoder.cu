@@ -17,12 +17,14 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
 #include <map>
 #include <vector>
 
 #include "attention.cuh"
 #include "attn_bwd_long.cuh"
 #include "common.h"
+#include "dropout.cuh"
 #include "encoder_bwd.cuh"
 #include "gemm_store.cuh"
 
@@ -53,9 +55,11 @@ struct EmbedParams {
                             // len[b] real tokens are written, kbias is left alone (all zero)
   int long_pad;             // packing: a sequence longer than 128 also writes its padding tokens up to a multiple of
                             // this many rows (0: none), see pack_chunk
+  drop::Cfg drop;           // kDrop: dropout of the LayerNorm output (site 0, dense batches only)
 };
 
-template <int NV, uint32_t FMT>  // H = NV * 256
+// kDrop: X0 = dropout(LN(E)), mask and scale applied in fp32 before the single 16-bit rounding
+template <int NV, uint32_t FMT, bool kDrop = false>  // H = NV * 256
 __global__ void __launch_bounds__(256) embed_ln_kernel(const EmbedParams p) {
   using A16 = act16::Act<FMT>;
   __shared__ int s_pos[512];
@@ -132,10 +136,22 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const EmbedParams p) {
       const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
       const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
       uint32_t h2[4];
+      if constexpr (kDrop) {
+        const uint4 w = drop::hidden_bits(p.drop, static_cast<uint32_t>(tok), v * 32 + lane);
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        h2[q] = A16::pack2((x[v * 8 + q * 2] - mean) * rstd * g[q * 2] + bb[q * 2],
-                           (x[v * 8 + q * 2 + 1] - mean) * rstd * g[q * 2 + 1] + bb[q * 2 + 1]);
+        for (int q = 0; q < 4; ++q) {
+          const uint32_t wq = drop::word(w, q);
+          const float y0 = (x[v * 8 + q * 2] - mean) * rstd * g[q * 2] + bb[q * 2];
+          const float y1 = (x[v * 8 + q * 2 + 1] - mean) * rstd * g[q * 2 + 1] + bb[q * 2 + 1];
+          h2[q] = A16::pack2(drop::keep(wq, 0, p.drop.thr) ? y0 * p.drop.scale : 0.f,
+                             drop::keep(wq, 1, p.drop.thr) ? y1 * p.drop.scale : 0.f);
+        }
+      } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          h2[q] = A16::pack2((x[v * 8 + q * 2] - mean) * rstd * g[q * 2] + bb[q * 2],
+                             (x[v * 8 + q * 2 + 1] - mean) * rstd * g[q * 2 + 1] + bb[q * 2 + 1]);
+      }
       out[v * 32 + lane] = make_uint4(h2[0], h2[1], h2[2], h2[3]);
     }
     if (lane == 0 && !varlen) {
@@ -441,7 +457,13 @@ struct ance_encoder {
   int varlen_align = 1;      // ance_encoder_forward_varlen / _packed: 1 = densest, 16 = exact packing, see pack_chunk
   std::vector<void*> allocs;
   // training (ance_encoder_forward_train / _backward)
-  std::map<const void*, int2> train_shapes;   // workspace -> (B, L) of a forward_train whose backward has not run yet
+  // workspace -> (B, L) and dropout (rates, seed) of a forward_train whose backward has not run yet
+  struct TrainRecord {
+    int B, L;
+    float p_hidden, p_attn;
+    uint64_t seed;
+  };
+  std::map<const void*, TrainRecord> train_shapes;
   int train_max_len = 128;                    // ance_encoder_set_param("train_max_len"): longest L the training calls accept
   struct LayerT { uint16_t *wqkv, *wo, *w1, *w2; };   // bf16 W^T: [H,3H] [H,H] [H,F] [F,H]
   std::vector<LayerT> wt;                     // empty until the first backward
@@ -502,12 +524,13 @@ int gelu_form() {
 // one GEMM of the forward: C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ R); act is the epilogue's code: 0 none, 1 / 2 GELU
 // (see gelu_form).  128 x 128 tile per CTA (the wgmma warpgroup holds the whole tile in registers: 128 fp32 accumulators
 // per thread), 4 operand stages, 4 epilogue warps reading the shared accumulator tile while the next tile is computed.
-template <uint32_t FMT>
+// kDrop: dropout of the bias output before the residual (EpStore), site and mask rows as *dc says
+template <uint32_t FMT, bool kDrop = false>
 int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
            const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls = ance::kClsGemm,
-           size_t ldr = 0) {
+           size_t ldr = 0, const drop::Cfg* dc = nullptr) {
   constexpr int BN = 128, CG = 1, EW = 4, STAGES = 4;
-  using Ep = gemm::EpStore<BN, EW, FMT>;
+  using Ep = gemm::EpStore<BN, EW, FMT, kDrop>;
   CUtensorMap tmA, tmB;
   if (!tc05_host::make_tmap_2d_16b(&tmA, A, M, K, lda, gemm::BM) || !tc05_host::make_tmap_2d_16b(&tmB, W, N, K, K, BN / CG)) {
     ance::set_error("encoder: cuTensorMapEncodeTiled failed (M=%d N=%d K=%d)", M, N, K);
@@ -533,6 +556,7 @@ int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K
   p.ldc32 = N;
   p.ldr = static_cast<int>(ldr);
   p.act = act;
+  if constexpr (kDrop) p.drop = *dc;
   {
     ance::ProfScope ps(cls, st);
     ANCE_CUDA((gemm::launch<Ep, BN, STAGES, CG, EW, FMT>(tmA, tmB, ws, p, 0, st)));
@@ -579,6 +603,9 @@ int set_attention_attrs() {
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<false, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<true, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<false, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<true, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<false, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   return ANCE_OK;
 }
 
@@ -620,10 +647,15 @@ int make_attention(AttentionLaunch& a, const uint16_t* qkv, uint16_t* ctx, int n
   return ANCE_OK;
 }
 
-template <uint32_t FMT>
+// kDrop: the dropout kernels (dense plans only; a.ap.drop filled in)
+template <uint32_t FMT, bool kDrop = false>
 int run_attention(const AttentionLaunch& a, cudaStream_t st) {
   ance::prof_begin(ance::kClsAttn, st);
-  if (a.single && a.packed) attn::attention_single_kernel<true, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  if constexpr (kDrop) {
+    if (a.single && a.packed) attn::attention_single_kernel<true, FMT, true><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+    else if (a.single) attn::attention_single_kernel<false, FMT, true><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+    else attn::attention_multi_kernel<false, FMT, true><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+  } else if (a.single && a.packed) attn::attention_single_kernel<true, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   else if (a.single) attn::attention_single_kernel<false, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   else if (a.packed) attn::attention_multi_kernel<true, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   else attn::attention_multi_kernel<false, FMT><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
@@ -680,6 +712,25 @@ struct TrainSave {
   float* head_in() const { return reinterpret_cast<float*>(ws + lo.head_in); }
 };
 
+// Dropout of a training forward (ance_encoder_forward_train_dropout): the rates and the seed; a rate of 0 runs that
+// site's kernels without dropout, so p_hidden = p_attn = 0 is ance_encoder_forward_train exactly.
+struct DropState {
+  float p_hidden = 0.f, p_attn = 0.f;
+  uint64_t seed = 0;
+  bool hidden() const { return p_hidden > 0.f; }
+  bool attn() const { return p_attn > 0.f; }
+  drop::Cfg cfg(float p, uint32_t site, int layer, int tok_stride = 1) const {
+    drop::Cfg c;
+    c.k0 = static_cast<uint32_t>(seed);
+    c.k1 = static_cast<uint32_t>(seed >> 32);
+    c.thr = static_cast<uint32_t>(std::min(lrint(static_cast<double>(p) * 65536.0), 65535L));
+    c.scale = 1.0f / (1.0f - static_cast<float>(c.thr) / 65536.0f);
+    c.stream = drop::stream(site, layer);
+    c.tok_stride = tok_stride;
+    return c;
+  }
+};
+
 // n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
 // token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
 // ts != null (dense, L <= the handle's train_max_len): the training forward — the same launches on the same inputs, with every activation the
@@ -687,7 +738,8 @@ struct TrainSave {
 // GEMM once more without GELU for the pre-activation), and the last layer always pruned to the CLS rows.
 template <uint32_t FMT>
 int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev, int B, int L,
-                 float* out_dev, cudaStream_t st, int n_tiles = 0, const TrainSave* ts = nullptr) {
+                 float* out_dev, cudaStream_t st, int n_tiles = 0, const TrainSave* ts = nullptr,
+                 const DropState* dr = nullptr) {
   const ance_encoder_config& c = e->cfg;
   const bool varlen = n_tiles > 0;
   const bool varlen_long = varlen && L > attn::kTile;   // sequences may span several tiles: multi-block attention items
@@ -709,12 +761,23 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   ep.X = ts ? ts->x(0) : e->X; ep.kbias = ts ? ts->kbias() : e->kbias; ep.err_flag = e->err_flag;
   ep.seq_row0 = varlen ? e->seq_row0 : nullptr;
   ep.long_pad = (varlen_long && e->varlen_align == 16) ? 32 : 0;
+  const bool drop_h = dr && dr->hidden(), drop_a = dr && dr->attn();
   ance::prof_begin(ance::kClsNorm, st);
-  switch (H / 256) {
-    case 1: embed_ln_kernel<1, FMT><<<B, 256, 0, st>>>(ep); break;
-    case 2: embed_ln_kernel<2, FMT><<<B, 256, 0, st>>>(ep); break;
-    case 3: embed_ln_kernel<3, FMT><<<B, 256, 0, st>>>(ep); break;
-    default: embed_ln_kernel<4, FMT><<<B, 256, 0, st>>>(ep); break;
+  if (drop_h) {
+    ep.drop = dr->cfg(dr->p_hidden, drop::kSiteEmbed, 0);
+    switch (H / 256) {
+      case 1: embed_ln_kernel<1, FMT, true><<<B, 256, 0, st>>>(ep); break;
+      case 2: embed_ln_kernel<2, FMT, true><<<B, 256, 0, st>>>(ep); break;
+      case 3: embed_ln_kernel<3, FMT, true><<<B, 256, 0, st>>>(ep); break;
+      default: embed_ln_kernel<4, FMT, true><<<B, 256, 0, st>>>(ep); break;
+    }
+  } else {
+    switch (H / 256) {
+      case 1: embed_ln_kernel<1, FMT><<<B, 256, 0, st>>>(ep); break;
+      case 2: embed_ln_kernel<2, FMT><<<B, 256, 0, st>>>(ep); break;
+      case 3: embed_ln_kernel<3, FMT><<<B, 256, 0, st>>>(ep); break;
+      default: embed_ln_kernel<4, FMT><<<B, 256, 0, st>>>(ep); break;
+    }
   }
   ance::prof_end(ance::kClsNorm, st);
   ANCE_CUDA(cudaGetLastError());
@@ -735,7 +798,12 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
     uint16_t* X_out = ts ? ts->x(l + 1) : e->X;
     if (ts && (rc = make_attention(attn_launch, QKV, CTX, M, L, c.heads, ts->kbias(), nullptr, nullptr, nullptr))) return rc;
     if ((rc = linear<FMT>(X_in, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
-    if ((rc = run_attention<FMT>(attn_launch, st))) return rc;
+    if (drop_a) {
+      attn_launch.ap.drop = dr->cfg(dr->p_attn, drop::kSiteAttn, l);
+      if ((rc = run_attention<FMT, true>(attn_launch, st))) return rc;
+    } else if ((rc = run_attention<FMT>(attn_launch, st))) {
+      return rc;
+    }
     // In the last layer only token 0 of every sequence is read downstream (models.py:49,193): run the
     // out-projection, FFN and both LayerNorms on those B rows only (strided TMA views, compact outputs).
     const bool cls_only = (e->prune_last_layer || varlen || ts) && (l == c.n_layer - 1);
@@ -750,11 +818,18 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
       ance::count_launch(2);
       ctx_a = e->cls_ctx; res_x = e->cls_x; pitch = H;
     }
-    if ((rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch))) return rc;
+    // dropout sites 2 and 3: row r of the pruned last layer is token r * L
+    const drop::Cfg dc_out = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, cls_only ? L : 1) : drop::Cfg{};
+    const drop::Cfg dc_ffn = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, cls_only ? L : 1) : drop::Cfg{};
+    if (drop_h) rc = linear<FMT, true>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch, &dc_out);
+    else rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch);
+    if (rc) return rc;
     if ((rc = layer_norm<FMT>(T1, false, H, Mr, H, d.ln1g, d.ln1b, c.ln_eps, X1, nullptr, st))) return rc;
     if (ts && (rc = linear<FMT>(X1, H, Mr, d.w1, F, H, d.b1, nullptr, 0, ts->at(l, ts->lo.u), nullptr, st, ance::kClsGemmFfn1))) return rc;
     if ((rc = linear<FMT>(X1, H, Mr, d.w1, F, H, d.b1, nullptr, gelu_form(), FF, nullptr, st, ance::kClsGemmFfn1))) return rc;
-    if ((rc = linear<FMT>(FF, F, Mr, d.w2, H, F, d.b2, X1, 0, T2, nullptr, st, ance::kClsGemmFfn2))) return rc;
+    if (drop_h) rc = linear<FMT, true>(FF, F, Mr, d.w2, H, F, d.b2, X1, 0, T2, nullptr, st, ance::kClsGemmFfn2, 0, &dc_ffn);
+    else rc = linear<FMT>(FF, F, Mr, d.w2, H, F, d.b2, X1, 0, T2, nullptr, st, ance::kClsGemmFfn2);
+    if (rc) return rc;
     if ((rc = layer_norm<FMT>(T2, false, H, Mr, H, d.ln2g, d.ln2b, c.ln_eps, X_out, nullptr, st))) return rc;
     if (e->dbg && M <= e->dbg_tokens)  // with cls_only the first B rows hold the CLS rows of the last layer
       ANCE_CUDA(cudaMemcpyAsync(e->dbg + static_cast<size_t>(l + 1) * e->dbg_tokens * H, X_out, static_cast<size_t>(Mr) * H * 2, cudaMemcpyDeviceToDevice, st));
@@ -971,13 +1046,16 @@ int ln_bwd(const void* x, bool in_f32, size_t x_ld, int rows, int H, const float
   return ANCE_OK;
 }
 
+// dc != null: the forward dropped the probabilities with this site (the kDrop kernels)
 template <uint32_t FMT>
 int attn_bwd(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, int B, int L,
-             int heads, cudaStream_t st) {
+             int heads, cudaStream_t st, const drop::Cfg* dc = nullptr) {
   const size_t smem = bwd::attn_bwd_smem(L);
   ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
+  ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
   ance::ProfScope ps(ance::kClsAttn, st);
-  bwd::attn_bwd_kernel<FMT><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f);
+  if (dc) bwd::attn_bwd_kernel<FMT, true><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f, *dc);
+  else bwd::attn_bwd_kernel<FMT><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f, drop::Cfg{});
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);
   return ANCE_OK;
@@ -986,13 +1064,55 @@ int attn_bwd(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool
 // L in {256, 384, 512}: the key-blocked kernels of attn_bwd_long.cuh; stats: bwdl::stats_floats(B, L, heads) fp32
 template <uint32_t FMT>
 int attn_bwd_long(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, float* stats,
-                  int B, int L, int heads, cudaStream_t st) {
+                  int B, int L, int heads, cudaStream_t st, const drop::Cfg* dc = nullptr) {
   const dim3 grid(L / bwdl::kBlk, heads, B);
   ance::ProfScope ps(ance::kClsAttn, st);
-  bwdl::dq_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f);
-  bwdl::dkv_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f);
+  if (dc) {
+    bwdl::dq_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, *dc);
+    bwdl::dkv_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, *dc);
+  } else {
+    bwdl::dq_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, drop::Cfg{});
+    bwdl::dkv_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, drop::Cfg{});
+  }
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(2);
+  return ANCE_OK;
+}
+
+// src * mask * scale over rows of H fp32 (row r is token r * tok_stride): the backward of a hidden dropout site
+// (in place allowed: src == dst)
+__global__ void __launch_bounds__(256) dropout_mask_rows_kernel(const float* src, float* dst, int rows, int H, const drop::Cfg c) {
+  const int groups = H / 8;
+  const size_t n = static_cast<size_t>(rows) * groups;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int r = static_cast<int>(i / groups), g = static_cast<int>(i % groups);
+    const uint4 w = drop::hidden_bits(c, static_cast<uint32_t>(r) * c.tok_stride, g);
+    const float4* s = reinterpret_cast<const float4*>(src + static_cast<size_t>(r) * H + g * 8);
+    float4* d = reinterpret_cast<float4*>(dst + static_cast<size_t>(r) * H + g * 8);
+    const float4 a = s[0], b = s[1];
+    d[0] = make_float4(drop::keep(w.x, 0, c.thr) ? a.x * c.scale : 0.f, drop::keep(w.x, 1, c.thr) ? a.y * c.scale : 0.f,
+                       drop::keep(w.y, 0, c.thr) ? a.z * c.scale : 0.f, drop::keep(w.y, 1, c.thr) ? a.w * c.scale : 0.f);
+    d[1] = make_float4(drop::keep(w.z, 0, c.thr) ? b.x * c.scale : 0.f, drop::keep(w.z, 1, c.thr) ? b.y * c.scale : 0.f,
+                       drop::keep(w.w, 0, c.thr) ? b.z * c.scale : 0.f, drop::keep(w.w, 1, c.thr) ? b.w * c.scale : 0.f);
+  }
+}
+
+// raw generator output (test hook): call i has the counter (low, high 32 bits of first + i, low, high 32 bits of
+// stream_word) and writes out[4 i .. 4 i + 3]
+__global__ void dropout_bits_kernel(uint32_t k0, uint32_t k1, uint64_t stream_word, uint64_t first, int64_t n, uint32_t* __restrict__ out) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t x = first + static_cast<uint64_t>(i);
+    const uint4 w = drop::philox(k0, k1, static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32), static_cast<uint32_t>(stream_word),
+                           static_cast<uint32_t>(stream_word >> 32));
+    reinterpret_cast<uint4*>(out)[i] = w;
+  }
+}
+
+// dst = src o mask * scale over rows of H fp32 (row r = token r * c.tok_stride): the backward of a hidden dropout site
+int mask_rows(const float* src, float* dst, int rows, int H, const drop::Cfg& c, cudaStream_t st) {
+  dropout_mask_rows_kernel<<<ew_grid(static_cast<size_t>(rows) * H / 8), 256, 0, st>>>(src, dst, rows, H, c);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
   return ANCE_OK;
 }
 
@@ -1076,9 +1196,12 @@ int wgrad(const uint16_t* dYt, int n_out, const uint16_t* Xt, int k_in, int rows
   return linear<kBF>(dYt, rows_p, n_out, Xt, k_in, rows_p, nullptr, nullptr, 0, nullptr, C32, st);
 }
 
+// dr: the dropout of the forward (null or zero rates: none).  At a hidden site T = m o Y s + R, the residual R gets the
+// LayerNorm's dT and the branch (bias, wgrad, dgrad) m o dT s; the embedding LayerNorm gets m o dX0 s.
 template <uint32_t FMT>
 int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws, const ance_encoder_grads* g,
-                  cudaStream_t st) {
+                  cudaStream_t st, const DropState* dr = nullptr) {
+  const bool drop_h = dr && dr->hidden(), drop_a = dr && dr->attn();
   const ance_encoder_config& c = e->cfg;
   const int H = c.hidden, F = c.ffn, M = B * L, Mp = (M + 7) / 8 * 8, NL = c.n_layer;
   constexpr int S = src_code<FMT>();
@@ -1112,10 +1235,17 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     const ance_layer_grads& lg = g->layers[l];
     const bool last = l == NL - 1;
     const int Mr = last ? B : M, Mrp = (Mr + 7) / 8 * 8;
-    // s.G = d X_out [Mr, H].  LN2: T2 = FF W2^T + b2 + X1
-    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t2), false, H, Mr, H, d.ln2g, c.ln_eps, s.G, s.dT, s.part, lg.ln2_g, lg.ln2_b, lg.ff2_b, st))) return rc;
-    if ((rc = to_bf16(s.dT, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
-    if ((rc = transpose_bf16<2>(s.dT, H, Mr, H, s.Gt, Mrp, st))) return rc;
+    // s.G = d X_out [Mr, H].  LN2: T2 = FF W2^T + b2 + X1  (dropout: T2 = m o (FF W2^T + b2) s + X1, the branch's
+    // gradient m o dT s goes to s.dX1, free until the FFN dgrad writes it)
+    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t2), false, H, Mr, H, d.ln2g, c.ln_eps, s.G, s.dT, s.part, lg.ln2_g, lg.ln2_b, drop_h ? nullptr : lg.ff2_b, st))) return rc;
+    const float* dT2 = s.dT;
+    if (drop_h) {
+      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, last ? L : 1), st))) return rc;
+      if ((rc = colsum(s.dX1, Mr, H, s.part, H, lg.ff2_b, nullptr, nullptr, st))) return rc;
+      dT2 = s.dX1;
+    }
+    if ((rc = to_bf16(dT2, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(dT2, H, Mr, H, s.Gt, Mrp, st))) return rc;
     if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.ff), F, Mr, F, s.Xt, Mrp, st))) return rc;
     if ((rc = wgrad(s.Gt, H, s.Xt, F, Mrp, lg.ff2_w, st))) return rc;
     if ((rc = linear<kBF>(s.A16, H, Mr, wt.w2, F, H, nullptr, nullptr, 0, nullptr, s.dA, st))) return rc;   // d FF
@@ -1133,15 +1263,22 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     if ((rc = linear<kBF>(s.A16, F, Mr, wt.w1, H, F, nullptr, nullptr, 0, nullptr, s.dX1, st))) return rc;   // d X1 (FFN)
     if ((rc = add_rows(s.dX1, 1, s.dT, Mr, H, st))) return rc;                                              // + residual
     // LN1: T1 = CTX Wo^T + bo + X_in
-    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t1), false, H, Mr, H, d.ln1g, c.ln_eps, s.dX1, s.dT, s.part, lg.ln1_g, lg.ln1_b, lg.ao_b, st))) return rc;
-    if ((rc = to_bf16(s.dT, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
-    if ((rc = transpose_bf16<2>(s.dT, H, Mr, H, s.Gt, Mrp, st))) return rc;
+    if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t1), false, H, Mr, H, d.ln1g, c.ln_eps, s.dX1, s.dT, s.part, lg.ln1_g, lg.ln1_b, drop_h ? nullptr : lg.ao_b, st))) return rc;
+    const float* dT1 = s.dT;
+    if (drop_h) {   // (s.dX1 was the LayerNorm's last input)
+      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, last ? L : 1), st))) return rc;
+      if ((rc = colsum(s.dX1, Mr, H, s.part, H, lg.ao_b, nullptr, nullptr, st))) return rc;
+      dT1 = s.dX1;
+    }
+    if ((rc = to_bf16(dT1, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
+    if ((rc = transpose_bf16<2>(dT1, H, Mr, H, s.Gt, Mrp, st))) return rc;
     if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.ctx), last ? static_cast<size_t>(L) * H : H, Mr, H, s.Xt, Mrp, st))) return rc;
     if ((rc = wgrad(s.Gt, H, s.Xt, H, Mrp, lg.ao_w, st))) return rc;
     if ((rc = linear<kBF>(s.A16, H, Mr, wt.wo, H, H, nullptr, nullptr, 0, s.dCTX, nullptr, st))) return rc;  // d CTX (bf16)
     // attention -> d QKV [M, 3H]
-    if (L <= attn::kTile) rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st);
-    else rc = attn_bwd_long<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, s.attn_stats, B, L, c.heads, st);
+    const drop::Cfg dca = drop_a ? dr->cfg(dr->p_attn, drop::kSiteAttn, l) : drop::Cfg{};
+    if (L <= attn::kTile) rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st, drop_a ? &dca : nullptr);
+    else rc = attn_bwd_long<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, s.attn_stats, B, L, c.heads, st, drop_a ? &dca : nullptr);
     if (rc) return rc;
     if ((rc = colsum(s.dA, M, 3 * H, s.part, H, lg.q_b, lg.k_b, lg.v_b, st))) return rc;
     if ((rc = to_bf16(s.dA, s.A16, static_cast<size_t>(M) * 3 * H, st))) return rc;
@@ -1165,6 +1302,7 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
   ANCE_CUDA(cudaMemsetAsync(g->word_emb, 0, static_cast<size_t>(c.vocab) * H * 4, st));
   ANCE_CUDA(cudaMemsetAsync(g->pos_emb, 0, static_cast<size_t>(c.max_pos) * H * 4, st));
   ANCE_CUDA(cudaMemsetAsync(g->type_emb, 0, static_cast<size_t>(c.type_vocab) * H * 4, st));
+  if (drop_h && (rc = mask_rows(s.G, s.G, M, H, dr->cfg(dr->p_hidden, drop::kSiteEmbed, 0), st))) return rc;
   if ((rc = ln_bwd<FMT>(s.dA, true, H, M, H, e->eg, c.ln_eps, s.G, s.dT, s.part, g->emb_ln_g, g->emb_ln_b, g->type_emb, st))) return rc;
   {
     ance::ProfScope ps(ance::kClsNorm, st);
@@ -1287,27 +1425,49 @@ extern "C" int ance_encoder_train_workspace(ance_encoder_t e, int B, int L, size
   return ANCE_OK;
 }
 
-extern "C" int ance_encoder_forward_train(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
-                                          const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev, void* stream) {
-  ANCE_REQUIRE(e != nullptr, "ance_encoder_forward_train: null handle");
-  ANCE_REQUIRE(ids_dev && out_dev && ws_dev, "ance_encoder_forward_train: null buffer");
-  ANCE_REQUIRE((lens_dev != nullptr) != (mask_dev != nullptr), "ance_encoder_forward_train: pass exactly one of lens_dev / mask_dev");
-  ANCE_REQUIRE(B > 0 && L > 0, "ance_encoder_forward_train: empty batch");
-  if (const int rc = check_train_len(e, L, "ance_encoder_forward_train")) return rc;
-  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(ws_dev) & 255u) == 0, "ance_encoder_forward_train: the workspace must be 256-byte aligned");
+namespace {
+
+int forward_train_impl(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev, int B, int L,
+                       void* ws_dev, float* out_dev, void* stream, const DropState& dr, const char* fn) {
+  ANCE_REQUIRE(e != nullptr, "%s: null handle", fn);
+  ANCE_REQUIRE(ids_dev && out_dev && ws_dev, "%s: null buffer", fn);
+  ANCE_REQUIRE((lens_dev != nullptr) != (mask_dev != nullptr), "%s: pass exactly one of lens_dev / mask_dev", fn);
+  ANCE_REQUIRE(B > 0 && L > 0, "%s: empty batch", fn);
+  if (const int rc = check_train_len(e, L, fn)) return rc;
+  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(ws_dev) & 255u) == 0, "%s: the workspace must be 256-byte aligned", fn);
   const ance_encoder_config& c = e->cfg;
-  ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "ance_encoder_forward_train: L = %d exceeds max_position_embeddings %d", L, c.max_pos);
+  ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "%s: L = %d exceeds max_position_embeddings %d", fn, L, c.max_pos);
   const long long tokens = static_cast<long long>(B) * L;
-  ANCE_REQUIRE(tokens <= e->max_tokens, "ance_encoder_forward_train: %lld tokens exceed max_tokens %d", tokens, e->max_tokens);
-  ANCE_REQUIRE(B <= e->max_tokens / 16, "ance_encoder_forward_train: batch %d too large for the head buffer", B);
+  ANCE_REQUIRE(tokens <= e->max_tokens, "%s: %lld tokens exceed max_tokens %d", fn, tokens, e->max_tokens);
+  ANCE_REQUIRE(B <= e->max_tokens / 16, "%s: batch %d too large for the head buffer", fn, B);
   int dev = -1;
   ANCE_CUDA(cudaGetDevice(&dev));
-  ANCE_REQUIRE(dev == e->device, "ance_encoder_forward_train: the handle belongs to device %d but device %d is current", e->device, dev);
+  ANCE_REQUIRE(dev == e->device, "%s: the handle belongs to device %d but device %d is current", fn, e->device, dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const TrainSave ts{reinterpret_cast<uint8_t*>(ws_dev), train_layout(c, B, L), c.n_layer};
-  e->train_shapes[ws_dev] = make_int2(B, L);
-  if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts);
-  return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts);
+  e->train_shapes[ws_dev] = ance_encoder::TrainRecord{B, L, dr.p_hidden, dr.p_attn, dr.seed};
+  if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts, &dr);
+  return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts, &dr);
+}
+
+}  // namespace
+
+extern "C" int ance_encoder_forward_train(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
+                                          const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev, void* stream) {
+  return forward_train_impl(e, ids_dev, lens_dev, mask_dev, B, L, ws_dev, out_dev, stream, DropState{}, "ance_encoder_forward_train");
+}
+
+extern "C" int ance_encoder_forward_train_dropout(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
+                                                  const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev,
+                                                  float p_hidden, float p_attn, uint64_t seed, void* stream) {
+  ANCE_REQUIRE(std::isfinite(p_hidden) && p_hidden >= 0.f && p_hidden < 1.f && std::isfinite(p_attn) && p_attn >= 0.f && p_attn < 1.f,
+               "ance_encoder_forward_train_dropout: dropout rates must be finite and in [0, 1) (p_hidden = %g, p_attn = %g)",
+               static_cast<double>(p_hidden), static_cast<double>(p_attn));
+  DropState dr;
+  dr.p_hidden = p_hidden;
+  dr.p_attn = p_attn;
+  dr.seed = seed;
+  return forward_train_impl(e, ids_dev, lens_dev, mask_dev, B, L, ws_dev, out_dev, stream, dr, "ance_encoder_forward_train_dropout");
 }
 
 extern "C" int ance_encoder_backward(ance_encoder_t e, const float* d_out_dev, void* ws_dev, const ance_encoder_grads* g,
@@ -1326,10 +1486,14 @@ extern "C" int ance_encoder_backward(ance_encoder_t e, const float* d_out_dev, v
   ANCE_REQUIRE(dev == e->device, "ance_encoder_backward: the handle belongs to device %d but device %d is current", e->device, dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   auto* ws = reinterpret_cast<uint8_t*>(ws_dev);
-  const int2 shape = it->second;
+  const ance_encoder::TrainRecord rec = it->second;
   e->train_shapes.erase(it);   // one backward per forward_train: the record cannot outlive the caller's workspace
-  if (e->fmt == tc05::kFmtBF16) return backward_impl<tc05::kFmtBF16>(e, shape.x, shape.y, d_out_dev, ws, g, st);
-  return backward_impl<tc05::kFmtF16>(e, shape.x, shape.y, d_out_dev, ws, g, st);
+  DropState dr;
+  dr.p_hidden = rec.p_hidden;
+  dr.p_attn = rec.p_attn;
+  dr.seed = rec.seed;
+  if (e->fmt == tc05::kFmtBF16) return backward_impl<tc05::kFmtBF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr);
+  return backward_impl<tc05::kFmtF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr);
 }
 
 extern "C" int ance_encoder_update_weights(ance_encoder_t e, const ance_encoder_weights* w_dev, void* stream) {
@@ -1757,6 +1921,39 @@ extern "C" int ance_dbg_attention_backward_long(int fmt, const void* qkv_dev, co
   return rc;
 }
 
+extern "C" int ance_dbg_attention_backward_dropout(int fmt, const void* qkv_dev, const float* kbias_dev,
+                                                   const void* dout_bf16_dev, int cls_only, int B, int L, int heads,
+                                                   float p_attn, uint64_t seed, int layer, float* dqkv_dev, void* stream) {
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "ance_dbg_attention_backward_dropout: unknown operand format %d", fmt);
+  ANCE_REQUIRE(qkv_dev && kbias_dev && dout_bf16_dev && dqkv_dev, "ance_dbg_attention_backward_dropout: null buffer");
+  ANCE_REQUIRE(aligned16(qkv_dev) && aligned16(dout_bf16_dev) && aligned16(dqkv_dev),
+               "ance_dbg_attention_backward_dropout: qkv, dout and dqkv must be 16-byte aligned");
+  ANCE_REQUIRE(heads >= 1 && heads <= 16, "ance_dbg_attention_backward_dropout: heads = %d outside [1, 16]", heads);
+  ANCE_REQUIRE(B > 0 && (L == 256 || L == 384 || L == 512 || (L > 0 && L <= attn::kTile)),
+               "ance_dbg_attention_backward_dropout: need B > 0 and 0 < L <= 128 or L in {256, 384, 512} (B = %d, L = %d)", B, L);
+  ANCE_REQUIRE(std::isfinite(p_attn) && p_attn > 0.f && p_attn < 1.f && layer >= 0,
+               "ance_dbg_attention_backward_dropout: need 0 < p_attn < 1 and layer >= 0 (p_attn = %g, layer = %d)",
+               static_cast<double>(p_attn), layer);
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* qkv = reinterpret_cast<const uint16_t*>(qkv_dev);
+  const auto* dout = reinterpret_cast<const uint16_t*>(dout_bf16_dev);
+  DropState dr;
+  dr.p_attn = p_attn;
+  dr.seed = seed;
+  const drop::Cfg dc = dr.cfg(p_attn, drop::kSiteAttn, layer);
+  const bool bf = fmt == ANCE_FMT_BF16;
+  if (L <= attn::kTile)
+    return bf ? attn_bwd<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st, &dc)
+              : attn_bwd<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st, &dc);
+  float* stats = nullptr;
+  ANCE_CUDA(cudaMallocAsync(&stats, bwdl::stats_floats(B, L, heads) * 4, st));
+  const int rc = bf ? attn_bwd_long<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st, &dc)
+                    : attn_bwd_long<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st, &dc);
+  ANCE_CUDA(cudaFreeAsync(stats, st));
+  return rc;
+}
+
 extern "C" int ance_dbg_layer_norm_backward(int fmt, const void* in_dev, int in_f32, int64_t in_ld, int rows, int H,
                                             const float* gamma_dev, float eps, const float* dy_dev, float* dx_dev,
                                             float* dgamma_dev, float* dbeta_dev, float* dsum_dev, void* stream) {
@@ -1811,6 +2008,19 @@ extern "C" int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L,
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(2);
   ANCE_CUDA(cudaFreeAsync(pos_ids, st));
+  return ANCE_OK;
+}
+
+extern "C" int ance_dbg_dropout_bits(uint64_t seed, uint64_t stream_word, uint64_t first_counter, int64_t n, uint32_t* out_dev,
+                                     void* stream) {
+  ANCE_REQUIRE(out_dev != nullptr && n > 0, "ance_dbg_dropout_bits: null buffer or n <= 0");
+  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(out_dev) & 15u) == 0, "ance_dbg_dropout_bits: out must be 16-byte aligned");
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  dropout_bits_kernel<<<ew_grid(static_cast<size_t>(n)), 256, 0, st>>>(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32),
+                                                                     stream_word, first_counter, n, out_dev);
+  ANCE_CUDA(cudaGetLastError());
+  ance::count_launch(1);
   return ANCE_OK;
 }
 

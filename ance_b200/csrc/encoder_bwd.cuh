@@ -12,6 +12,7 @@
 //   refresh_kernel       in-place weight refresh (ance_encoder_update_weights) in one launch
 #pragma once
 #include "act16.cuh"
+#include "dropout.cuh"
 
 namespace bwd {
 
@@ -35,10 +36,14 @@ __device__ __forceinline__ uint16_t float_to_bf16(float f) { return __bfloat16_a
 constexpr int kAttnPitch = 65;
 inline size_t attn_bwd_smem(int L) { return (static_cast<size_t>(4) * L * kAttnPitch + static_cast<size_t>(L) * (L + 1)) * 4; }
 
-template <uint32_t FMT>
+// kDrop: the forward dropped probabilities with the mask m of site 1 and scale s (dropout.cuh): P~ = m o P s,
+// dP = m o (dO V^T) s, dV = P~^T dO, D = sum_j P dP, dS = P o (dP - D).  The mask is generated once, with P, and kept as
+// the sign bit of P's shared-memory entry (P >= 0; a dropped P is stored negated, -0 for 0).
+template <uint32_t FMT, bool kDrop = false>
 __global__ void __launch_bounds__(256) attn_bwd_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                        const uint16_t* __restrict__ dout, int cls_only,
-                                                       float* __restrict__ dqkv, int L, int heads, float scale_log2) {
+                                                       float* __restrict__ dqkv, int L, int heads, float scale_log2,
+                                                       const drop::Cfg dc) {
   using A16 = act16::Act<FMT>;
   extern __shared__ float sm[];
   const int b = blockIdx.x, h = blockIdx.y, H = heads * 64;
@@ -89,9 +94,21 @@ __global__ void __launch_bounds__(256) attn_bwd_kernel(const uint16_t* __restric
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
     const float inv = 1.f / sum;
+    if constexpr (kDrop) {
 #pragma unroll
-    for (int t = 0; t < 4; ++t)
-      if (lane + 32 * t < L) sP[i * PP + lane + 32 * t] = s[t] * inv;
+      for (int t = 0; t < 4; ++t) {
+        const int j = lane + 32 * t;
+        if (j < L) {
+          const uint4 w = drop::philox(dc.k0, dc.k1, 4u * t + ((j >> 1) & 3), i, b * heads + h, dc.stream);
+          const float pv = s[t] * inv;
+          sP[i * PP + j] = drop::keep(drop::word(w, (j >> 3) & 3), j & 1, dc.thr) ? pv : __uint_as_float(__float_as_uint(pv) | 0x80000000u);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int t = 0; t < 4; ++t)
+        if (lane + 32 * t < L) sP[i * PP + lane + 32 * t] = s[t] * inv;
+    }
   }
   __syncthreads();
   // [L, 64] outputs: thread (r0, d) owns rows r0 + 4k, column d; within a warp r0 is uniform (the P / dS reads broadcast)
@@ -104,11 +121,11 @@ __global__ void __launch_bounds__(256) attn_bwd_kernel(const uint16_t* __restric
     const float o = sO[i * kAttnPitch + d];
 #pragma unroll
     for (int k = 0; k < 32; ++k)
-      if (r0 + 4 * k < L) acc[k] = fmaf(sP[i * PP + r0 + 4 * k], o, acc[k]);
+      if (r0 + 4 * k < L) acc[k] = fmaf(kDrop ? fmaxf(sP[i * PP + r0 + 4 * k], 0.f) : sP[i * PP + r0 + 4 * k], o, acc[k]);
   }
 #pragma unroll
   for (int k = 0; k < 32; ++k)
-    if (r0 + 4 * k < L) dqkv[(tok0 + r0 + 4 * k) * 3 * H + 2 * H + h * 64 + d] = acc[k];
+    if (r0 + 4 * k < L) dqkv[(tok0 + r0 + 4 * k) * 3 * H + 2 * H + h * 64 + d] = kDrop ? acc[k] * dc.scale : acc[k];
   __syncthreads();
   // dS / 8 over P: one warp per row
   for (int i = warp; i < L; i += 8) {
@@ -122,9 +139,16 @@ __global__ void __launch_bounds__(256) attn_bwd_kernel(const uint16_t* __restric
         float a = 0.f;
 #pragma unroll 16
         for (int c = 0; c < 64; ++c) a = fmaf(sO[i * kAttnPitch + c], sV[j * kAttnPitch + c], a);
-        dp[t] = a;
-        p[t] = sP[i * PP + j];
-        dsum = fmaf(p[t], a, dsum);
+        if constexpr (kDrop) {
+          const float pm = sP[i * PP + j];
+          dp[t] = signbit(pm) ? 0.f : a * dc.scale;
+          p[t] = fabsf(pm);
+          dsum = fmaf(p[t], dp[t], dsum);
+        } else {
+          dp[t] = a;
+          p[t] = sP[i * PP + j];
+          dsum = fmaf(p[t], a, dsum);
+        }
       }
     }
 #pragma unroll

@@ -10,6 +10,7 @@
 // asynchronously under the next slab's math.  Rows / columns past the tensor edge are clipped by TMA.
 #pragma once
 #include "act16.cuh"
+#include "dropout.cuh"
 #include "gemm_core.cuh"
 
 namespace gemm {
@@ -93,8 +94,9 @@ __device__ __forceinline__ void gelu_logistic2(float& x0, float& x1) {
 }
 
 // FMT: 16-bit format of the OUTPUT and of the residual (act16.cuh); the operand format of the GEMM itself is the
-// FMT parameter of gemm::launch.
-template <int BN, int EPI_WARPS, uint32_t FMT = tc05::kFmtBF16>
+// FMT parameter of gemm::launch.  kDrop: dropout between the bias (and activation) and the residual, in fp32 before the
+// one rounding: C = m o (A W^T + bias) / (1 - p) + R, the mask of output row r being that of token r * drop.tok_stride.
+template <int BN, int EPI_WARPS, uint32_t FMT = tc05::kFmtBF16, bool kDrop = false>
 struct EpStore {
   using A16 = act16::Act<FMT>;
   static constexpr uint64_t kHintA = tc05::kEvictNormal;
@@ -114,6 +116,7 @@ struct EpStore {
     const uint16_t* R;       // residual [M, ldr] (FMT) or null
     int ldc, ldc32, ldr;
     int act;                 // 0 none, 1 gelu (erfc form, |err| <= 7e-7), 2 gelu (logistic form, |err| <= 3.7e-6)
+    drop::Cfg drop;          // kDrop only
   };
 
   uint32_t rphase;
@@ -158,6 +161,18 @@ struct EpStore {
     } else if (p.act == 2) {
 #pragma unroll
       for (int i = 0; i < 32; i += 2) gelu_logistic2(f[i], f[i + 1]);
+    }
+    if constexpr (kDrop) {
+      if (row_ok) {
+        const uint32_t t = static_cast<uint32_t>(row) * static_cast<uint32_t>(p.drop.tok_stride);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint4 w = drop::hidden_bits(p.drop, t, static_cast<uint32_t>(col0 >> 3) + k);
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            f[8 * k + i] = drop::keep(drop::word(w, i >> 1), i & 1, p.drop.thr) ? f[8 * k + i] * p.drop.scale : 0.f;
+        }
+      }
     }
     if (direct_residual && p.R && row_ok) {
       const uint16_t* r = p.R + (size_t)row * p.ldr + col0;

@@ -14,7 +14,9 @@ libance_b200.so (csrc/encoder.cu).  There is no CPU path — calling them with C
 Training: after ``model.set_trainable(True)`` (inputs of up to 128 tokens) or ``model.set_trainable(True, max_len=512)``
 (up to 512: FirstP documents, MaxP chunks; DPR's BiEncoder needs ``max_len=256``) ``query_emb`` / ``body_emb`` /
 ``forward()`` build an autograd graph whose backward runs the encoder's own backward kernels, so ``loss.backward()``
-fills the parameters' ``.grad``; by default the outputs carry no graph.
+fills the parameters' ``.grad``; by default the outputs carry no graph.  ``set_trainable(True, ..., dropout=True)`` adds
+the reference's training-mode dropout (hidden and attention-probability rates from the config; 0.1 for DPR) while the
+module is in ``train()`` mode.
 """
 from __future__ import annotations
 
@@ -231,19 +233,25 @@ class _CudaEncoder:
         self.__dict__.pop("_allpad", None)   # values cached per weights
         return True
 
-    def forward_train(self, ids: torch.Tensor, lens: Optional[torch.Tensor], mask: Optional[torch.Tensor]):
+    def forward_train(self, ids: torch.Tensor, lens: Optional[torch.Tensor], mask: Optional[torch.Tensor],
+                      dropout: Optional[tuple] = None):
         """forward() of a whole [B, L] batch (L <= 128, or a multiple of 128 up to the handle's train_max_len) that also
-        keeps what the backward needs.  -> (out fp32 [B, H],
-        workspace tensor for backward())."""
+        keeps what the backward needs; dropout = (p_hidden, p_attn, seed) runs it in training mode
+        (ance_encoder_forward_train_dropout).  -> (out fp32 [B, H], workspace tensor for backward())."""
         B, L = ids.shape
         n = C.c_size_t()
         _lib.check(self.lib.ance_encoder_train_workspace(self.h, B, L, C.byref(n)))
         ws = torch.empty(n.value, dtype=torch.uint8, device=ids.device)
         out = torch.empty((B, self.hidden_size), dtype=torch.float32, device=ids.device)
+        args = (self.h, ids.data_ptr(), None if lens is None else lens.data_ptr(), None if mask is None else mask.data_ptr(),
+                B, L, ws.data_ptr(), out.data_ptr())
         with torch.cuda.device(ids.device):
-            _lib.check(self.lib.ance_encoder_forward_train(
-                self.h, ids.data_ptr(), None if lens is None else lens.data_ptr(),
-                None if mask is None else mask.data_ptr(), B, L, ws.data_ptr(), out.data_ptr(), _lib.current_stream()))
+            if dropout is None:
+                _lib.check(self.lib.ance_encoder_forward_train(*args, _lib.current_stream()))
+            else:
+                p_hidden, p_attn, seed = dropout
+                _lib.check(self.lib.ance_encoder_forward_train_dropout(*args, float(p_hidden), float(p_attn), int(seed),
+                                                                       _lib.current_stream()))
         return out, ws
 
     def backward(self, d_out: torch.Tensor, ws: torch.Tensor, grads) -> None:
@@ -260,8 +268,8 @@ class _TrainableEncode(torch.autograd.Function):
     _param_groups order), so that their .grad accumulates and DDP's hooks fire."""
 
     @staticmethod
-    def forward(ctx, enc, n_layer, ids, lens, mask, *params):
-        out, ws = enc.forward_train(ids, lens, mask)
+    def forward(ctx, enc, n_layer, ids, lens, mask, dropout, *params):
+        out, ws = enc.forward_train(ids, lens, mask, dropout)
         ctx.enc, ctx.ws, ctx.n_layer = enc, ws, n_layer
         ctx.shapes = [p.shape for p in params]
         return out
@@ -274,7 +282,7 @@ class _TrainableEncode(torch.autograd.Function):
         n = ctx.n_layer
         groups = (flat[:5], [flat[5 + 16 * i:5 + 16 * (i + 1)] for i in range(n)], flat[5 + 16 * n:])
         ctx.enc.backward(d_out.float().contiguous(), ctx.ws, groups)
-        return (None, None, None, None, None, *flat)
+        return (None, None, None, None, None, None, *flat)
 
 
 def _forward_varlen(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
@@ -330,17 +338,44 @@ class _B200Encoder(nn.Module):
     #: set_trainable(True): embeddings computed while grad is enabled carry an autograd graph (dense, L <= _train_max_len)
     _trainable = False
     _train_max_len = 128
+    _dropout = (0.0, 0.0)   # (hidden, attention-probability) rates of the trainable forward in train() mode
 
-    def set_trainable(self, on: bool = True, max_len: int = 128):
+    def _default_dropout(self) -> tuple:
+        """dropout=True: the checkpoint config's hidden_dropout_prob / attention_probs_dropout_prob."""
+        return (float(self.config.hidden_dropout_prob), float(self.config.attention_probs_dropout_prob))
+
+    def set_trainable(self, on: bool = True, max_len: int = 128, dropout=False):
         """Opt in to gradients: while torch grad mode is on, query_emb / body_emb / encode_lens (dense batches of up to
         `max_len` tokens per sequence or MaxP chunk: 8, 16, 32, 64 or 128, or a multiple of 128 up to max_len) and the
         triplet forward() return tensors whose backward runs the encoder's backward kernels; the other encode paths raise
-        instead of returning detached results.  max_len is 128, 256, 384 or 512.  Off by default."""
+        instead of returning detached results.  max_len is 128, 256, 384 or 512.  Off by default.
+
+        dropout: False (default) trains the eval-mode forward; True applies the reference's training-mode dropout with the
+        rates of the config (RoBERTa: hidden_dropout_prob / attention_probs_dropout_prob; the DPR BiEncoder: 0.1 / 0.1);
+        a float sets both rates.  Dropout is applied only on the gradient path and only while the module is in train()
+        mode (from_pretrained ends in eval()); each encode draws its mask seed from torch's default CPU generator, so
+        torch.manual_seed reproduces a step."""
         if max_len not in (128, 256, 384, 512):
             raise ValueError(f"max_len must be 128, 256, 384 or 512, got {max_len!r}")
+        if dropout is True:
+            rates = self._default_dropout()
+        elif dropout is False or dropout is None:
+            rates = (0.0, 0.0)
+        else:
+            rates = (float(dropout), float(dropout))
+        if not all(0.0 <= r < 1.0 for r in rates):
+            raise ValueError(f"dropout rates must be in [0, 1), got {rates!r}")
         self._trainable = bool(on)
         self._train_max_len = int(max_len)
+        self._dropout = rates
         return self
+
+    def _train_dropout(self) -> Optional[tuple]:
+        """(p_hidden, p_attn, seed) for one trainable encode, or None (no dropout configured, or eval() mode)."""
+        if not self.training or self._dropout == (0.0, 0.0):
+            return None
+        lo, hi = torch.randint(0, 2 ** 32, (2,), dtype=torch.int64).tolist()
+        return self._dropout + (lo | (hi << 32),)
 
     def _grad_path(self) -> bool:
         return self._trainable and torch.is_grad_enabled()
@@ -372,7 +407,7 @@ class _B200Encoder(nn.Module):
             enc._train_max_len = max_len
         embs, layers, hd = _param_groups(backbone, head)
         params = embs + [t for l in layers for t in l] + hd
-        return _TrainableEncode.apply(enc, len(layers), ids, lens, mask, *params)
+        return _TrainableEncode.apply(enc, len(layers), ids, lens, mask, self._train_dropout(), *params)
 
     def _enc_for(self, name, backbone, arch, heads, pad_id, head, device) -> _CudaEncoder:
         if device.type != "cuda":
@@ -675,13 +710,16 @@ class BiEncoder(_B200Encoder):
         self.ctx_model = _backbone(d.vocab_size, d.hidden_size, d.num_hidden_layers, d.intermediate_size,
                                    d.max_position_embeddings, d.type_vocab_size, d.pad_token_id, d.layer_norm_eps)
 
-    def set_trainable(self, on: bool = True, max_len: Optional[int] = None):
+    def set_trainable(self, on: bool = True, max_len: Optional[int] = None, dropout=False):
         """As _B200Encoder.set_trainable for both BERT encoders; training needs an explicit max_len (DPR's inputs are 256
-        tokens: set_trainable(True, max_len=256))."""
+        tokens: set_trainable(True, max_len=256)).  dropout=True is HFBertEncoder.init_encoder's default rate, 0.1."""
         if on and max_len is None:
             raise NotImplementedError("the DPR BiEncoder trains on 256-token inputs: call set_trainable(True, max_len=256) "
                                       "(or 128 / 384 / 512 for other input lengths)")
-        return super().set_trainable(on, 128 if max_len is None else max_len)
+        return super().set_trainable(on, 128 if max_len is None else max_len, dropout)
+
+    def _default_dropout(self) -> tuple:
+        return (0.1, 0.1)   # model/models.py:229-233, init_encoder(dropout=0.1)
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         # HF BertModel checkpoints carry pooler.* and position_ids buffers the path never uses

@@ -254,6 +254,17 @@ int ance_encoder_train_workspace(ance_encoder_t enc, int B, int L, size_t* bytes
  * B * L <= max_tokens. */
 int ance_encoder_forward_train(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev,
                                int B, int L, void* ws_dev, float* out_dev, void* stream);
+/* ance_encoder_forward_train in training mode: inverted dropout (keep with probability 1 - p, kept values scaled by
+ * 1 / (1 - p)) at the four sites of a BERT / RoBERTa layer stack in training mode: the embedding LayerNorm's output, the
+ * attention probabilities (p_attn), and the attention-output and FFN-output projections before their residual adds
+ * (p_hidden); not the head.  Masks are regenerated from `seed` by a counter-based generator (Philox4x32-10) as functions of
+ * the logical element (site, layer, token, column; layer, sequence, head, query, key), so the backward needs no stored mask:
+ * ance_encoder_backward applies the masks this call used.  16 bits per decision: the effective rate is round(p 2^16) / 2^16.
+ * Each rate must be finite and in [0, 1) (else ANCE_ERR_INVALID); a rate of 0 turns its sites off, and both 0 is
+ * ance_encoder_forward_train exactly. */
+int ance_encoder_forward_train_dropout(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev,
+                                       const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev, float p_hidden,
+                                       float p_attn, uint64_t seed, void* stream);
 /* Gradients of sum(d_out o out) with respect to every weight, for the forward that filled ws_dev (the weights must not
  * have changed since).  d_out_dev [B, hidden] fp32, 16-byte aligned.  The handle forgets ws_dev once this call is made:
  * a second backward from the same workspace is ANCE_ERR_INVALID.  Backward GEMM operands are bf16 whatever operand_fmt is, with fp32
@@ -355,6 +366,17 @@ int ance_dbg_embedding_backward(const int32_t* ids_dev, int B, int L, int H, int
  * columns R .. dst_ld - 1 of dst set to zero. */
 int ance_dbg_transpose_bf16(int src_kind, const void* src_dev, int64_t src_ld, int R, int C, void* dst_dev, int64_t dst_ld,
                             void* stream);
+/* The dropout generator's raw output: n Philox4x32-10 calls under the key (seed & 0xffffffff, seed >> 32); call i has
+ * the counter (lo32(first_counter + i), hi32(first_counter + i), lo32(stream_word), hi32(stream_word)) and writes its four
+ * words to out_dev[4 i .. 4 i + 3] (device, 16-byte aligned). */
+int ance_dbg_dropout_bits(uint64_t seed, uint64_t stream_word, uint64_t first_counter, int64_t n, uint32_t* out_dev, void* stream);
+/* The backward's attention kernels with dropout (what ance_encoder_backward launches after
+ * ance_encoder_forward_train_dropout): the arguments of ance_dbg_attention_backward (L <= 128) or
+ * ance_dbg_attention_backward_long (L in {256, 384, 512}), plus the probability rate p_attn (finite, in (0, 1)), the seed
+ * and the layer whose site-1 mask to apply. */
+int ance_dbg_attention_backward_dropout(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                        int cls_only, int B, int L, int heads, float p_attn, uint64_t seed, int layer,
+                                        float* dqkv_dev, void* stream);
 /* Host-only: the byte offsets of the workspace ance_encoder_forward_train fills for a [B, L] batch (L <= 128, or a multiple
  * of 128 up to the handle's "train_max_len"), out[15] =
  * ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total.  ids [B * L] int32 and kbias

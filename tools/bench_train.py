@@ -5,10 +5,13 @@ eager autograd of the oracle (oracle/encoder_oracle.py, TF32 off) on the same GP
   maxp    rdot_nll_multi_chunk, 2 triplets, queries of 64, documents of 4 chunks x 512 (MaxP)
   dpr     the DPR BiEncoder (two BERTs), 16 (question, passage) pairs at 256 with in-batch negatives  Prints one JSON line with the median step times, the card's name,
 its power limit and the median SM clock sampled during the timed steps; also the same loss without a graph (the inference
-forward) and, with --profile, our step's device time per kernel class from a separate run.
+forward) and, with --profile, our step's device time per kernel class from a separate run.  --dropout instead times our
+step with the reference's training-mode dropout (set_trainable(..., dropout=True): 0.1 at every site) and without it,
+alternating in --rounds rounds of --steps steps within one process, and prints both medians and every round's median
+(with --profile also the device time per kernel class of each, from separate runs).
 
     python tools/bench_train.py [--workload psg|firstp|maxp|dpr] [--layers 12] [--steps 20] [--warmup 5]
-                                [--fmt fp16|bf16] [--profile]
+                                [--fmt fp16|bf16] [--profile] [--dropout [--rounds 3]]
 """
 import argparse
 import json
@@ -120,7 +123,7 @@ def _setup(workload, layers, fmt):
                 t.grad = None
             _in_batch(orc[0]._hidden_states(*q)[-1][:, 0], orc[1]._hidden_states(*a)[-1][:, 0]).backward()
 
-        return ours, ours_forward, oracle
+        return ours, ours_forward, oracle, model
     cfg = roberta_base_config(num_hidden_layers=layers)
     sd = random_roberta_state_dict(seed=0, n_layer=layers)
     model = (RobertaDot_CLF_ANN_NLL_MultiChunk if workload == "maxp" else RobertaDot_NLL_LN)(cfg)
@@ -163,7 +166,7 @@ def _setup(workload, layers, fmt):
         else:
             _nll(emb(*q), emb(*a), emb(*b)).backward()
 
-    return ours, ours_forward, oracle
+    return ours, ours_forward, oracle, model
 
 
 def _nll(q, a, b):
@@ -192,10 +195,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--fmt", default="fp16", choices=("fp16", "bf16"))
     ap.add_argument("--profile", action="store_true", help="also report our step's device time per kernel class")
+    ap.add_argument("--dropout", action="store_true", help="time our step with and without dropout, alternating")
+    ap.add_argument("--rounds", type=int, default=3, help="--dropout: rounds of (off, on)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train needs a GPU")
-    ours, ours_forward, oracle = _setup(args.workload, args.layers, args.fmt)
+    ours, ours_forward, oracle, model = _setup(args.workload, args.layers, args.fmt)
+    if args.dropout:
+        return _dropout_ab(args, ours, model)
 
     prev = torch.backends.cuda.matmul.allow_tf32
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -224,6 +231,42 @@ def main():
         "sm_clock_mhz_median": statistics.median(clk.samples) if clk.samples else None,
         "steps": args.steps, "warmup": args.warmup,
         "profile_ms_and_launches_per_step": profile}))
+
+
+def _dropout_ab(args, ours, model):
+    model.train()
+    max_len = model._train_max_len
+    rounds = {False: [], True: []}
+    with ClockSampler() as clk:
+        for _ in range(args.rounds):
+            for on in (False, True):
+                model.set_trainable(True, max_len=max_len, dropout=on)
+                rounds[on].append(_time(ours, args.steps, args.warmup)[0])
+    off, on = statistics.median(rounds[False]), statistics.median(rounds[True])
+    profile = {}
+    if args.profile:   # separate, untimed runs: device time per kernel class with dropout off and on
+        for flag in (False, True):
+            model.set_trainable(True, max_len=max_len, dropout=flag)
+            _lib.profile_enable(True)
+            _lib.profile_read(reset=True)
+            for _ in range(args.steps):
+                ours()
+            torch.cuda.synchronize()
+            profile["dropout" if flag else "no_dropout"] = {k: round(ms / args.steps, 3) for k, (ms, n) in
+                                                            _lib.profile_read().items() if n}
+            _lib.profile_enable(False)
+    name, power = _smi("name,power.limit").split(", ")
+    print(json.dumps({
+        "workload": f"{WORKLOADS[args.workload]}, {args.layers} layers, hidden 768", "operand_fmt": args.fmt,
+        "dropout": model._dropout if hasattr(model, "_dropout") else None,
+        "step_ms_median_no_dropout": round(off, 3), "step_ms_median_dropout": round(on, 3),
+        "dropout_cost_pct": round(100 * (on - off) / off, 2),
+        "round_medians_no_dropout": [round(x, 3) for x in rounds[False]],
+        "round_medians_dropout": [round(x, 3) for x in rounds[True]],
+        "gpu": name, "power_limit_w": float(power),
+        "sm_clock_mhz_median": statistics.median(clk.samples) if clk.samples else None,
+        "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds,
+        "profile_ms_per_step": profile or None}))
 
 
 if __name__ == "__main__":
