@@ -109,6 +109,9 @@ SIGNATURES = {
     "ance_encoder_forward_train_dropout": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                                      C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_uint64,
                                                      C.c_void_p]),
+    "ance_encoder_train_workspace_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ance_encoder_forward_train_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                    C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_uint64, C.c_void_p]),
     "ance_encoder_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(EncoderGrads), C.c_void_p]),
     "ance_encoder_update_weights": (C.c_int, [C.c_void_p, C.POINTER(EncoderWeights), C.c_void_p]),
     "ance_encoder_debug_grads": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -118,6 +121,11 @@ SIGNATURES = {
                                        C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ance_dbg_pack_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "ance_dbg_attention_backward_packed": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_uint64,
+                                                     C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_dbg_pack_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ance_dbg_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                 C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ance_dbg_linear": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,

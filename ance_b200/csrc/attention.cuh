@@ -58,9 +58,13 @@ struct Params {
   const int32_t* row_hi;
   // attention_multi_kernel<kPacked = true>: per 128-row tile, (first key row, number of 128-key blocks) of its work items
   const int2* tile_kv;
-  // kDrop kernels (dense sequences only, row_lo null): dropout of the probabilities, site 1 (dropout.cuh).  The dropped
-  // entries of the 16-bit P are zero, the row sum l keeps every p, and ctx = O * (drop.scale / l).
+  // kDrop kernels: dropout of the probabilities, site 1 (dropout.cuh).  The dropped entries of the 16-bit P are zero, the
+  // row sum l keeps every p, and ctx = O * (drop.scale / l).  With a row plan the counters are those of the dense batch:
+  // row_tok[r] = b seq_L + i is the token of row r (-1: no sequence), its keys are counted from row_lo[r]; the plan's
+  // sequences start at multiples of 8 rows (varlen_align 16).
   drop::Cfg drop;
+  const int32_t* row_tok;
+  int seq_L;
 };
 
 struct Smem {
@@ -204,9 +208,15 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
       // end of the whole 32-key chunks of the own sequence (counted from its first key): the keys the dense kernel,
       // with the sequence at key 0, handles in unmasked chunks
       const int seq_full = seq_lo + ((seq_hi - seq_lo) & ~31);
-      // kDrop (dense, L >= 256): this row is query qi of sequence tok / L; its keys are the item's kv0 .. kv0 + L - 1
-      const uint32_t d_qi = kDrop ? static_cast<uint32_t>((tok0 + row) % p.L) : 0u;
-      const uint32_t d_c2 = kDrop ? static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h) : 0u;
+      // kDrop (dense, L >= 256): this row is query qi of sequence tok / L; its keys are the item's kv0 .. kv0 + L - 1.
+      // kDrop with a row plan: query and sequence from row_tok, keys counted from the row's own first key.
+      uint32_t d_qi = kDrop ? static_cast<uint32_t>((tok0 + row) % p.L) : 0u;
+      uint32_t d_c2 = kDrop ? static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h) : 0u;
+      if (kDrop && kPacked) {
+        const int tk = max(__ldg(p.row_tok + tok0 + row), 0);
+        d_qi = static_cast<uint32_t>(tk % p.seq_L);
+        d_c2 = static_cast<uint32_t>((tk / p.seq_L) * p.heads + h);
+      }
       float m_run = -INFINITY, l_run = 0.f;
       float o[kDh];
 #pragma unroll
@@ -296,7 +306,16 @@ attention_multi_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
               uint32_t v[32];
               acc_ld_x32(srow + c, v);
               uint4 dw[4];   // kDrop: the four calls of this 32-key chunk (dw[q] covers the key pairs q, q + 4, q + 8, q + 12)
-              if constexpr (kDrop) {
+              if constexpr (kDrop && kPacked) {   // key index of column c in the row's sequence: any multiple of 8
+                const int koff = j * kTile + c - seq_lo;
+                const int a = koff >> 5, r8 = (koff >> 3) & 3;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  const uint4 wa = drop::philox(p.drop.k0, p.drop.k1, 4u * static_cast<uint32_t>(a) + q, d_qi, d_c2, p.drop.stream);
+                  dw[q] = r8 == 0 ? wa : drop::splice(wa, drop::philox(p.drop.k0, p.drop.k1, 4u * static_cast<uint32_t>(a + 1) + q,
+                                                                       d_qi, d_c2, p.drop.stream), r8);
+                }
+              } else if constexpr (kDrop) {
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
                   dw[q] = drop::philox(p.drop.k0, p.drop.k1, 4u * static_cast<uint32_t>((j * kTile + c) >> 5) + q, d_qi, d_c2,
@@ -507,7 +526,7 @@ struct RowSt {
 };
 
 // kDrop: a row's dropout counter words: query index qi in its sequence, c2 = sequence * heads + head, and lo, the tile
-// column of the sequence's key 0
+// column of the sequence's key 0 (dense: a multiple of L; a row plan: a multiple of 8)
 struct DropRow {
   uint32_t qi, c2;
   int lo;
@@ -524,7 +543,11 @@ __device__ __forceinline__ uint4 drop_bits(const drop::Cfg& dc, const DropRow& r
     return rot == 0 ? w : rot == 1 ? make_uint4(w.w, w.x, w.y, w.z) : rot == 2 ? make_uint4(w.z, w.w, w.x, w.y)
                                                                                 : make_uint4(w.y, w.z, w.w, w.x);
   }
-  return drop::philox(dc.k0, dc.k1, 4u * static_cast<uint32_t>((32 * cc - r.lo) >> 5) + q4, r.qi, r.c2, dc.stream);
+  const int k0 = 32 * cc - r.lo;   // key index of column 32 cc in the row's sequence
+  const uint4 wa = drop::philox(dc.k0, dc.k1, 4u * static_cast<uint32_t>(k0 >> 5) + q4, r.qi, r.c2, dc.stream);
+  if ((k0 & 31) == 0) return wa;
+  return drop::splice(wa, drop::philox(dc.k0, dc.k1, 4u * static_cast<uint32_t>((k0 >> 5) + 1) + q4, r.qi, r.c2, dc.stream),
+                      (k0 >> 3) & 3);
 }
 
 // Softmax of the two rows (r, r + 8) held by accumulator `d` (m64n128 fragment): P packed in pairs into `pk` (the A
@@ -688,9 +711,16 @@ attention_single_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_
     for (int i = 0; i < 4; ++i) {
       const int row = r0 + (i & 1) * 8 + (i >> 1) * 64;
       if constexpr (kDrop) {
-        dr[i].qi = static_cast<uint32_t>((tok0 + row) % p.L);
-        dr[i].c2 = static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h);
-        dr[i].lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;
+        if (varlen) {
+          const int tk = max(__ldg(p.row_tok + tok0 + row), 0);
+          dr[i].qi = static_cast<uint32_t>(tk % p.seq_L);
+          dr[i].c2 = static_cast<uint32_t>((tk / p.seq_L) * p.heads + h);
+          dr[i].lo = __ldg(p.row_lo + tok0 + row) - tok0;
+        } else {
+          dr[i].qi = static_cast<uint32_t>((tok0 + row) % p.L);
+          dr[i].c2 = static_cast<uint32_t>(((tok0 + row) / p.L) * p.heads + h);
+          dr[i].lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;
+        }
       }
       int lo = (p.L >= kTile) ? 0 : (row / p.L) * p.L;   // keys of this row's own sequence
       int hi = (p.L >= kTile) ? kTile : lo + p.L;

@@ -16,6 +16,9 @@
 // converted to bf16).  Statistics, D and dS are fp32.  No key block is skipped.
 // With cls_only only token 0 of a sequence has an upstream gradient: dq_kernel writes zeros for query blocks > 0, and
 // dkv_kernel visits query block 0 only.
+// Packed row plans (kSeq: seq_row0 / seq_len): sequence b occupies the rows seq_row0[b] .. + seq_len[b] (the grid still
+// spans L / 64 blocks, and blocks that start at or past the length exit).  Rows past the length are read as zeros and never
+// written, and keys past it take the dense kernel's padding bias, so a row's arithmetic is that of the dense batch.
 // Each warp owns 16 rows of its CTA's 64; its products are 16 x 64 accumulator tiles whose fp32 fragments are re-packed
 // in registers as the A operand of the next product (the m16n8k16 C and A fragments share their row / column layout).
 #pragma once
@@ -127,10 +130,26 @@ __device__ __forceinline__ void load_tile(uint16_t* s, uint16_t* bf, const uint1
   }
 }
 
-// the dO tile of query block qb: rows of dout [B*L, H], or with cls_only the sequence's single row of dout [B, H]
-__device__ __forceinline__ void load_dout(uint16_t* s, const uint16_t* dout, int cls_only, int b, int L, int qb, int h, int H) {
+// the dO tile of query block qb: n_rows rows of dout [*, H] from row tok0 + 64 qb, or with cls_only the sequence's single
+// row of dout [B, H]
+__device__ __forceinline__ void load_dout(uint16_t* s, const uint16_t* dout, int cls_only, int b, size_t tok0, int n_rows,
+                                          int qb, int h, int H) {
   if (cls_only) load_tile<tc05::kFmtBF16>(s, nullptr, dout + static_cast<size_t>(b) * H + h * 64, H, qb == 0 ? 1 : 0);
-  else load_tile<tc05::kFmtBF16>(s, nullptr, dout + (static_cast<size_t>(b) * L + qb * kBlk) * H + h * 64, H, kBlk);
+  else load_tile<tc05::kFmtBF16>(s, nullptr, dout + (tok0 + qb * kBlk) * H + h * 64, H, n_rows);
+}
+
+// the key bias of key j (kSeq: the plan's, all zero, inside the sequence, the dense padding bias past its length)
+template <bool kSeq>
+__device__ __forceinline__ float key_bias(const float* kbias, size_t tok0, int j, int len) {
+  if constexpr (kSeq) return j < len ? kbias[tok0 + j] : -10000.0f * 1.4426950408889634f;
+  return kbias[tok0 + j];
+}
+
+// rows of block x (64 x .. 64 x + 63) inside the sequence
+template <bool kSeq>
+__device__ __forceinline__ int block_rows(int x, int len) {
+  if constexpr (kSeq) return min(kBlk, len - x * kBlk);
+  return kBlk;
 }
 
 // the max and sum over the 4 lanes of a quad (the lanes holding one accumulator row)
@@ -166,44 +185,50 @@ __device__ __forceinline__ void drop_dp_rows(float (&dp)[8][4], const drop::Cfg&
 }
 
 // accumulator element (n, e) of lane (g = lane / 4, t = lane % 4) sits at row g + 8 (e / 2), column 8 n + 2 t + e % 2
-template <uint32_t FMT, bool kDrop = false>
+template <uint32_t FMT, bool kDrop = false, bool kSeq = false>
 __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                       const uint16_t* __restrict__ dout, int cls_only,
                                                       float* __restrict__ dqkv, float* __restrict__ stats, int L,
-                                                      int heads, float scale_log2, const drop::Cfg dc) {
+                                                      int heads, float scale_log2, const drop::Cfg dc,
+                                                      const int32_t* __restrict__ seq_row0 = nullptr,
+                                                      const int32_t* __restrict__ seq_len = nullptr) {
   constexpr bool kConv = FMT == tc05::kFmtF16;
   __shared__ alignas(16) uint16_t sQ[kBlk * kPitch], sO[kBlk * kPitch], sK[kBlk * kPitch], sV[kBlk * kPitch];
   __shared__ alignas(16) uint16_t sKb_[kConv ? kBlk * kPitch : 8];
   __shared__ float sB[kBlk];
   uint16_t* sKb = kConv ? sKb_ : sK;
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z, H = heads * 64;
+  const int len = kSeq ? seq_len[b] : L;
+  if (kSeq && qb * kBlk >= len) return;   // these rows belong to no part of the sequence
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const size_t ld = static_cast<size_t>(3) * H, tok0 = static_cast<size_t>(b) * L;
-  const size_t row_a = tok0 + qb * kBlk + warp * 16 + g;   // this lane's rows: row_a and row_a + 8
+  const size_t ld = static_cast<size_t>(3) * H;
+  const size_t tok0 = kSeq ? static_cast<size_t>(seq_row0[b]) : static_cast<size_t>(b) * L;
+  const int ra = qb * kBlk + warp * 16 + g;                // this lane's rows in the sequence: ra and ra + 8
+  const size_t row_a = tok0 + ra;
   if (cls_only && qb > 0) {   // no upstream gradient in this block: dQ = 0
 #pragma unroll
     for (int n = 0; n < 8; ++n)
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf)
-        *reinterpret_cast<float2*>(dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t) = make_float2(0.f, 0.f);
+        if (!kSeq || ra + 8 * hf < len) *reinterpret_cast<float2*>(dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t) = make_float2(0.f, 0.f);
     return;
   }
-  load_tile<FMT>(sQ, nullptr, qkv + (tok0 + qb * kBlk) * ld + h * 64, ld, kBlk);
-  load_dout(sO, dout, cls_only, b, L, qb, h, H);
+  load_tile<FMT>(sQ, nullptr, qkv + (tok0 + qb * kBlk) * ld + h * 64, ld, block_rows<kSeq>(qb, len));
+  load_dout(sO, dout, cls_only, b, tok0, block_rows<kSeq>(qb, len), qb, h, H);
   __syncthreads();
   uint32_t aQ[4][4], aO[4][4];
   load_a(aQ, sQ, warp * 16, lane);
   load_a(aO, sO, warp * 16, lane);
-  const int nkb = L / kBlk;
+  const int nkb = kSeq ? (len + kBlk - 1) / kBlk : L / kBlk;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, dn[2] = {0.f, 0.f};
   float s[8][4], dp[8][4];
   // pass 1: m, l and sum_j exp2(s - m) dP over all keys, rescaled at every new maximum
   for (int kb = 0; kb < nkb; ++kb) {
     __syncthreads();
     const uint16_t* kv = qkv + (tok0 + kb * kBlk) * ld + h * 64;
-    load_tile<FMT>(sK, nullptr, kv + H, ld, kBlk);
-    load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, kBlk);   // V converted to bf16 in place
-    if (threadIdx.x < kBlk) sB[threadIdx.x] = kbias[tok0 + kb * kBlk + threadIdx.x];
+    load_tile<FMT>(sK, nullptr, kv + H, ld, block_rows<kSeq>(kb, len));
+    load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, block_rows<kSeq>(kb, len));   // V converted to bf16 in place
+    if (threadIdx.x < kBlk) sB[threadIdx.x] = key_bias<kSeq>(kbias, tok0, kb * kBlk + threadIdx.x, len);
     __syncthreads();
     zero(s);
     zero(dp);
@@ -254,9 +279,9 @@ __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict
   for (int kb = 0; kb < nkb; ++kb) {
     __syncthreads();
     const uint16_t* kv = qkv + (tok0 + kb * kBlk) * ld + h * 64;
-    load_tile<FMT>(sK, kConv ? sKb : nullptr, kv + H, ld, kBlk);
-    load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, kBlk);
-    if (threadIdx.x < kBlk) sB[threadIdx.x] = kbias[tok0 + kb * kBlk + threadIdx.x];
+    load_tile<FMT>(sK, kConv ? sKb : nullptr, kv + H, ld, block_rows<kSeq>(kb, len));
+    load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, block_rows<kSeq>(kb, len));
+    if (threadIdx.x < kBlk) sB[threadIdx.x] = key_bias<kSeq>(kbias, tok0, kb * kBlk + threadIdx.x, len);
     __syncthreads();
     zero(s);
     zero(dp);
@@ -279,39 +304,46 @@ __global__ void __launch_bounds__(kThreads) dq_kernel(const uint16_t* __restrict
   for (int n = 0; n < 8; ++n)
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf)
-      *reinterpret_cast<float2*>(dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t) = make_float2(dq[n][2 * hf], dq[n][2 * hf + 1]);
+      if (!kSeq || ra + 8 * hf < len)
+        *reinterpret_cast<float2*>(dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t) = make_float2(dq[n][2 * hf], dq[n][2 * hf + 1]);
 }
 
-template <uint32_t FMT, bool kDrop = false>
+template <uint32_t FMT, bool kDrop = false, bool kSeq = false>
 __global__ void __launch_bounds__(kThreads) dkv_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                        const uint16_t* __restrict__ dout, int cls_only,
                                                        float* __restrict__ dqkv, const float* __restrict__ stats, int L,
-                                                       int heads, float scale_log2, const drop::Cfg dc) {
+                                                       int heads, float scale_log2, const drop::Cfg dc,
+                                                       const int32_t* __restrict__ seq_row0 = nullptr,
+                                                       const int32_t* __restrict__ seq_len = nullptr) {
   constexpr bool kConv = FMT == tc05::kFmtF16;
   __shared__ alignas(16) uint16_t sQ[kBlk * kPitch], sO[kBlk * kPitch], sK[kBlk * kPitch], sV[kBlk * kPitch];
   __shared__ alignas(16) uint16_t sQb_[kConv ? kBlk * kPitch : 8];
   __shared__ float sM[kBlk], sI[kBlk], sD[kBlk];
   uint16_t* sQb = kConv ? sQb_ : sQ;
   const int kb = blockIdx.x, h = blockIdx.y, b = blockIdx.z, H = heads * 64;
+  const int len = kSeq ? seq_len[b] : L;
+  if (kSeq && kb * kBlk >= len) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const size_t ld = static_cast<size_t>(3) * H, tok0 = static_cast<size_t>(b) * L;
+  const size_t ld = static_cast<size_t>(3) * H;
+  const size_t tok0 = kSeq ? static_cast<size_t>(seq_row0[b]) : static_cast<size_t>(b) * L;
   const uint16_t* kv = qkv + (tok0 + kb * kBlk) * ld + h * 64;
-  load_tile<FMT>(sK, nullptr, kv + H, ld, kBlk);
-  load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, kBlk);
+  load_tile<FMT>(sK, nullptr, kv + H, ld, block_rows<kSeq>(kb, len));
+  load_tile<FMT>(sV, kConv ? sV : nullptr, kv + 2 * H, ld, block_rows<kSeq>(kb, len));
   __syncthreads();
   uint32_t aK[4][4], aV[4][4];
   load_a(aK, sK, warp * 16, lane);
   load_a(aV, sV, warp * 16, lane);
-  const float kb_r[2] = {kbias[tok0 + kb * kBlk + warp * 16 + g], kbias[tok0 + kb * kBlk + warp * 16 + g + 8]};
+  const int ka = kb * kBlk + warp * 16 + g;   // this lane's keys in the sequence: ka and ka + 8
+  const float kb_r[2] = {key_bias<kSeq>(kbias, tok0, ka, len), key_bias<kSeq>(kbias, tok0, ka + 8, len)};
   const float* st = stats + (static_cast<size_t>(b) * heads + h) * 3 * L;
   float dk[8][4], dv[8][4], s[8][4], dp[8][4];
   zero(dk);
   zero(dv);
-  const int nqb = cls_only ? 1 : L / kBlk;
+  const int nqb = cls_only ? 1 : kSeq ? (len + kBlk - 1) / kBlk : L / kBlk;
   for (int qb = 0; qb < nqb; ++qb) {
     __syncthreads();
-    load_tile<FMT>(sQ, kConv ? sQb : nullptr, qkv + (tok0 + qb * kBlk) * ld + h * 64, ld, kBlk);
-    load_dout(sO, dout, cls_only, b, L, qb, h, H);
+    load_tile<FMT>(sQ, kConv ? sQb : nullptr, qkv + (tok0 + qb * kBlk) * ld + h * 64, ld, block_rows<kSeq>(qb, len));
+    load_dout(sO, dout, cls_only, b, tok0, block_rows<kSeq>(qb, len), qb, h, H);
     if (threadIdx.x < kBlk) {
       sM[threadIdx.x] = st[qb * kBlk + threadIdx.x];
       sI[threadIdx.x] = st[L + qb * kBlk + threadIdx.x];
@@ -359,11 +391,12 @@ __global__ void __launch_bounds__(kThreads) dkv_kernel(const uint16_t* __restric
     acc_to_a(aP, dp);
     mma_ab(dk, aP, sQb, lane);
   }
-  const size_t row_a = tok0 + kb * kBlk + warp * 16 + g;
+  const size_t row_a = tok0 + ka;
 #pragma unroll
   for (int n = 0; n < 8; ++n)
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
+      if (kSeq && ka + 8 * hf >= len) continue;
       float* o = dqkv + (row_a + 8 * hf) * ld + h * 64 + n * 8 + 2 * t;
       *reinterpret_cast<float2*>(o + H) = make_float2(dk[n][2 * hf], dk[n][2 * hf + 1]);
       *reinterpret_cast<float2*>(o + 2 * H) = make_float2(dv[n][2 * hf], dv[n][2 * hf + 1]);

@@ -23,14 +23,20 @@ enum : uint32_t { kSiteEmbed = 0, kSiteAttn = 1, kSiteAttnOut = 2, kSiteFfnOut =
 __host__ __device__ constexpr uint32_t stream(uint32_t site, int layer) { return 4u * static_cast<uint32_t>(layer) + site; }
 
 // one dropout site of one launch: the Philox key, the threshold and scale, the counter word c3 (and, for the GEMM
-// epilogue, the token stride of its rows: 1, or L when row r is the CLS row of sequence r)
+// epilogue, the token stride of its rows: 1, or L when row r is the CLS row of sequence r; or, for a packed row plan, the
+// token b L + i of every row, -1 for a row of no sequence)
 struct Cfg {
   uint32_t k0, k1;
   uint32_t thr;
   uint32_t stream;
   float scale;
   int tok_stride;
+  const int32_t* row_tok;   // null: row r is token r * tok_stride
 };
+
+__host__ __device__ __forceinline__ uint32_t row_token(const Cfg& c, int r) {
+  return c.row_tok ? static_cast<uint32_t>(c.row_tok[r]) : static_cast<uint32_t>(r) * static_cast<uint32_t>(c.tok_stride);
+}
 
 __device__ __forceinline__ uint4 philox(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) {
 #pragma unroll
@@ -54,6 +60,15 @@ __device__ __forceinline__ uint32_t word(const uint4& w, int i) { return i == 0 
 
 // keep decision of the 16-bit half `half` of a generator word
 __device__ __forceinline__ bool keep(uint32_t w, int half, uint32_t thr) { return ((w >> (16 * half)) & 0xFFFFu) >= thr; }
+
+// Attention probabilities of keys whose index inside their sequence starts at a multiple of 8 but not of 32 (packed row
+// plans: a sequence's keys start at any multiple of 16 of a tile): the 32 keys k0 + 8 m + 2 q4 + {0, 1} (m = 0..3) of a
+// lane lie in the dense calls a = k0 >> 5 and a + 1; word m of the result is the word those keys use, with r = (k0 >> 3) & 3
+// words taken from call a and the rest from call a + 1.
+__device__ __forceinline__ uint4 splice(const uint4& wa, const uint4& wb, int r) {
+  return r == 0 ? wa : r == 1 ? make_uint4(wa.y, wa.z, wa.w, wb.x) : r == 2 ? make_uint4(wa.z, wa.w, wb.x, wb.y)
+                                                                             : make_uint4(wa.w, wb.x, wb.y, wb.z);
+}
 
 // the four words of the hidden-site call covering columns 8 g .. 8 g + 7 of token t
 __device__ __forceinline__ uint4 hidden_bits(const Cfg& c, uint32_t t, uint32_t g) { return philox(c.k0, c.k1, g, t, 0u, c.stream); }

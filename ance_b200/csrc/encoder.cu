@@ -55,7 +55,7 @@ struct EmbedParams {
                             // len[b] real tokens are written, kbias is left alone (all zero)
   int long_pad;             // packing: a sequence longer than 128 also writes its padding tokens up to a multiple of
                             // this many rows (0: none), see pack_chunk
-  drop::Cfg drop;           // kDrop: dropout of the LayerNorm output (site 0, dense batches only)
+  drop::Cfg drop;           // kDrop: dropout of the LayerNorm output (site 0), token t of sequence b counted as b L + t
 };
 
 // kDrop: X0 = dropout(LN(E)), mask and scale applied in fp32 before the single 16-bit rounding
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const EmbedParams p) {
       const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
       uint32_t h2[4];
       if constexpr (kDrop) {
-        const uint4 w = drop::hidden_bits(p.drop, static_cast<uint32_t>(tok), v * 32 + lane);
+        const uint4 w = drop::hidden_bits(p.drop, static_cast<uint32_t>(b * p.L + t), v * 32 + lane);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const uint32_t wq = drop::word(w, q);
@@ -462,6 +462,7 @@ struct ance_encoder {
     int B, L;
     float p_hidden, p_attn;
     uint64_t seed;
+    int n_tiles;   // 0: dense; else ance_encoder_forward_train_packed's plan of n_tiles * 128 rows (kept in the workspace)
   };
   std::map<const void*, TrainRecord> train_shapes;
   int train_max_len = 128;                    // ance_encoder_set_param("train_max_len"): longest L the training calls accept
@@ -606,6 +607,7 @@ int set_attention_attrs() {
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<false, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_single_kernel<true, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::SmemSingle::kDynamic));
   ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<false, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
+  ANCE_CUDA(cudaFuncSetAttribute(attn::attention_multi_kernel<true, FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn::Smem::kDynamic));
   return ANCE_OK;
 }
 
@@ -647,13 +649,14 @@ int make_attention(AttentionLaunch& a, const uint16_t* qkv, uint16_t* ctx, int n
   return ANCE_OK;
 }
 
-// kDrop: the dropout kernels (dense plans only; a.ap.drop filled in)
+// kDrop: the dropout kernels (a.ap.drop filled in; with a row plan also a.ap.row_tok / seq_L)
 template <uint32_t FMT, bool kDrop = false>
 int run_attention(const AttentionLaunch& a, cudaStream_t st) {
   ance::prof_begin(ance::kClsAttn, st);
   if constexpr (kDrop) {
     if (a.single && a.packed) attn::attention_single_kernel<true, FMT, true><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
     else if (a.single) attn::attention_single_kernel<false, FMT, true><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
+    else if (a.packed) attn::attention_multi_kernel<true, FMT, true><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
     else attn::attention_multi_kernel<false, FMT, true><<<a.grid, attn::kThreads, attn::Smem::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   } else if (a.single && a.packed) attn::attention_single_kernel<true, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
   else if (a.single) attn::attention_single_kernel<false, FMT><<<a.grid, attn::kSingleThreads, attn::SmemSingle::kDynamic, st>>>(a.tmQKV, a.tmCTX, a.ap);
@@ -676,12 +679,13 @@ struct TrainLayout {
 constexpr int kTrainLayoutFields = 15;   // ance_dbg_train_layout returns them in this order
 static_assert(sizeof(TrainLayout) == kTrainLayoutFields * sizeof(size_t), "ance_dbg_train_layout lists every field");
 
-TrainLayout train_layout(const ance_encoder_config& c, int B, int L) {
-  const size_t M = static_cast<size_t>(B) * L, H = c.hidden, F = c.ffn;
+// n_tiles > 0: a packed plan (ance_encoder_forward_train_packed): M = n_tiles * 128 rows, ids still the dense [B, L]
+TrainLayout train_layout(const ance_encoder_config& c, int B, int L, int n_tiles = 0) {
+  const size_t M = n_tiles > 0 ? static_cast<size_t>(n_tiles) * 128 : static_cast<size_t>(B) * L, H = c.hidden, F = c.ffn;
   auto up = [](size_t x) { return (x + 255) / 256 * 256; };
   TrainLayout t;
   size_t o = 0;
-  t.ids = o; o += up(M * 4);
+  t.ids = o; o += up(static_cast<size_t>(B) * L * 4);
   t.kbias = o; o += up(M * 4);
   t.layers = o;
   size_t p = 0;
@@ -701,16 +705,60 @@ TrainLayout train_layout(const ance_encoder_config& c, int B, int L) {
   return t;
 }
 
+// A packed training forward keeps, after the fields of train_layout, its row plan and the CLS rows its pruned last layer
+// gathered: seq_row0 [B], seq_len [B], row_lo / row_hi / row_tok [M] int32 (row_tok: token b L + i of each row, -1 for a
+// row of no sequence), tile_kv [n_tiles] int2, cls_ctx / cls_x [B, H] 16-bit.
+struct PackedLayout {
+  size_t seq_row0, seq_len, row_lo, row_hi, row_tok, tile_kv, cls_ctx, cls_x, total;
+};
+
+PackedLayout packed_layout(const ance_encoder_config& c, int B, int L, int n_tiles) {
+  auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t M = static_cast<size_t>(n_tiles) * 128;
+  PackedLayout p;
+  size_t o = train_layout(c, B, L, n_tiles).total;
+  p.seq_row0 = o; o += up(static_cast<size_t>(B) * 4);
+  p.seq_len = o; o += up(static_cast<size_t>(B) * 4);
+  p.row_lo = o; o += up(M * 4);
+  p.row_hi = o; o += up(M * 4);
+  p.row_tok = o; o += up(M * 4);
+  p.tile_kv = o; o += up(static_cast<size_t>(n_tiles) * 8);
+  p.cls_ctx = o; o += up(static_cast<size_t>(B) * c.hidden * 2);
+  p.cls_x = o; o += up(static_cast<size_t>(B) * c.hidden * 2);
+  p.total = o;
+  return p;
+}
+
 struct TrainSave {
   uint8_t* ws;
   TrainLayout lo;
   int n_layer;
+  // packed plans only (null: dense)
+  int32_t *seq_row0 = nullptr, *seq_len = nullptr, *row_lo = nullptr, *row_hi = nullptr, *row_tok = nullptr;
+  int2* tile_kv = nullptr;
+  uint16_t *cls_ctx = nullptr, *cls_x = nullptr;
   uint16_t* at(int l, size_t off) const { return reinterpret_cast<uint16_t*>(ws + lo.layers + l * lo.per_layer + off); }
   uint16_t* x(int l) const { return l == n_layer ? reinterpret_cast<uint16_t*>(ws + lo.x_final) : at(l, lo.x_in); }
   int32_t* ids() const { return reinterpret_cast<int32_t*>(ws + lo.ids); }
   float* kbias() const { return reinterpret_cast<float*>(ws + lo.kbias); }
   float* head_in() const { return reinterpret_cast<float*>(ws + lo.head_in); }
 };
+
+TrainSave train_save(const ance_encoder_config& c, uint8_t* ws, int B, int L, int n_tiles) {
+  TrainSave ts{ws, train_layout(c, B, L, n_tiles), c.n_layer};
+  if (n_tiles > 0) {
+    const PackedLayout p = packed_layout(c, B, L, n_tiles);
+    ts.seq_row0 = reinterpret_cast<int32_t*>(ws + p.seq_row0);
+    ts.seq_len = reinterpret_cast<int32_t*>(ws + p.seq_len);
+    ts.row_lo = reinterpret_cast<int32_t*>(ws + p.row_lo);
+    ts.row_hi = reinterpret_cast<int32_t*>(ws + p.row_hi);
+    ts.row_tok = reinterpret_cast<int32_t*>(ws + p.row_tok);
+    ts.tile_kv = reinterpret_cast<int2*>(ws + p.tile_kv);
+    ts.cls_ctx = reinterpret_cast<uint16_t*>(ws + p.cls_ctx);
+    ts.cls_x = reinterpret_cast<uint16_t*>(ws + p.cls_x);
+  }
+  return ts;
+}
 
 // Dropout of a training forward (ance_encoder_forward_train_dropout): the rates and the seed; a rate of 0 runs that
 // site's kernels without dropout, so p_hidden = p_attn = 0 is ance_encoder_forward_train exactly.
@@ -719,7 +767,7 @@ struct DropState {
   uint64_t seed = 0;
   bool hidden() const { return p_hidden > 0.f; }
   bool attn() const { return p_attn > 0.f; }
-  drop::Cfg cfg(float p, uint32_t site, int layer, int tok_stride = 1) const {
+  drop::Cfg cfg(float p, uint32_t site, int layer, int tok_stride = 1, const int32_t* row_tok = nullptr) const {
     drop::Cfg c;
     c.k0 = static_cast<uint32_t>(seed);
     c.k1 = static_cast<uint32_t>(seed >> 32);
@@ -727,15 +775,18 @@ struct DropState {
     c.scale = 1.0f / (1.0f - static_cast<float>(c.thr) / 65536.0f);
     c.stream = drop::stream(site, layer);
     c.tok_stride = tok_stride;
+    c.row_tok = row_tok;
     return c;
   }
 };
 
 // n_tiles > 0: variable-length packing — the plan (e->seq_row0 / row_lo / row_hi / tile_kv) is already on the device, the
 // token matrix has n_tiles * 128 rows and the CLS rows are gathered by index.  With L > 128 sequences may span tiles.
-// ts != null (dense, L <= the handle's train_max_len): the training forward — the same launches on the same inputs, with every activation the
+// ts != null (L <= the handle's train_max_len): the training forward — the same launches on the same inputs, with every activation the
 // backward needs written to its own slot of the workspace instead of the reused buffers of the handle (plus the FFN-up
-// GEMM once more without GELU for the pre-activation), and the last layer always pruned to the CLS rows.
+// GEMM once more without GELU for the pre-activation), and the last layer always pruned to the CLS rows.  With n_tiles > 0
+// as well, the plan and the gathered CLS rows are the workspace's (ts->seq_row0 ...), so that several training forwards
+// can precede their backwards; dropout masks are those of the dense batch (token b L + i, dropout.cuh).
 template <uint32_t FMT>
 int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_dev, const uint8_t* mask_dev, int B, int L,
                  float* out_dev, cudaStream_t st, int n_tiles = 0, const TrainSave* ts = nullptr,
@@ -744,22 +795,31 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   const bool varlen = n_tiles > 0;
   const bool varlen_long = varlen && L > attn::kTile;   // sequences may span several tiles: multi-block attention items
   const int M = varlen ? n_tiles * attn::kTile : B * L, H = c.hidden, F = c.ffn;
+  const bool own_plan = varlen && ts;   // the plan lives in the training workspace
+  const int32_t* seq_row0 = own_plan ? ts->seq_row0 : e->seq_row0;
+  const int32_t* row_lo = own_plan ? ts->row_lo : e->row_lo;
+  const int32_t* row_hi = own_plan ? ts->row_hi : e->row_hi;
+  const int2* tile_kv = own_plan ? ts->tile_kv : e->tile_kv;
+  uint16_t* cls_ctx = own_plan ? ts->cls_ctx : e->cls_ctx;
+  uint16_t* cls_x = own_plan ? ts->cls_x : e->cls_x;
+  const int32_t* row_tok = own_plan ? ts->row_tok : nullptr;
   int rc;
   if (varlen) {   // rows behind the last sequence of a tile: zeros (finite through every layer), no key bias anywhere
-    ANCE_CUDA(cudaMemsetAsync(e->X, 0, static_cast<size_t>(M) * H * 2, st));
-    ANCE_CUDA(cudaMemsetAsync(e->kbias, 0, static_cast<size_t>(M) * 4, st));
+    ANCE_CUDA(cudaMemsetAsync(ts ? ts->x(0) : e->X, 0, static_cast<size_t>(M) * H * 2, st));
+    ANCE_CUDA(cudaMemsetAsync(ts ? ts->kbias() : e->kbias, 0, static_cast<size_t>(M) * 4, st));
   }
   // K1
   EmbedParams ep;
-  if (ts) ANCE_CUDA(cudaMemcpyAsync(ts->ids(), ids_dev, static_cast<size_t>(M) * 4, cudaMemcpyDeviceToDevice, st));
-  ep.ids = ids_dev; ep.lens = lens_dev; ep.mask = mask_dev;
+  if (ts) ANCE_CUDA(cudaMemcpyAsync(ts->ids(), ids_dev, static_cast<size_t>(B) * L * 4, cudaMemcpyDeviceToDevice, st));
+  ep.ids = ids_dev; ep.mask = mask_dev;
+  ep.lens = own_plan ? ts->seq_len : lens_dev;   // (a packed training plan: the lengths it was planned from)
   ep.B = B; ep.L = L; ep.H = H;
   ep.roberta = (c.arch == ANCE_ARCH_ROBERTA);
   ep.pad_id = c.pad_id; ep.vocab = c.vocab; ep.max_pos = c.max_pos;
   ep.word = e->word; ep.pos = e->pos; ep.type = e->type;
   ep.gamma = e->eg; ep.beta = e->eb; ep.eps = c.ln_eps;
   ep.X = ts ? ts->x(0) : e->X; ep.kbias = ts ? ts->kbias() : e->kbias; ep.err_flag = e->err_flag;
-  ep.seq_row0 = varlen ? e->seq_row0 : nullptr;
+  ep.seq_row0 = varlen ? seq_row0 : nullptr;
   ep.long_pad = (varlen_long && e->varlen_align == 16) ? 32 : 0;
   const bool drop_h = dr && dr->hidden(), drop_a = dr && dr->attn();
   ance::prof_begin(ance::kClsNorm, st);
@@ -784,8 +844,8 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
   ance::count_launch(1);
   if (e->dbg && M <= e->dbg_tokens) ANCE_CUDA(cudaMemcpyAsync(e->dbg, e->X, static_cast<size_t>(M) * H * 2, cudaMemcpyDeviceToDevice, st));
   AttentionLaunch attn_launch;
-  if ((rc = make_attention(attn_launch, e->QKV, e->CTX, M, L, c.heads, e->kbias, varlen ? e->row_lo : nullptr,
-                           varlen ? e->row_hi : nullptr, varlen ? e->tile_kv : nullptr))) return rc;
+  if ((rc = make_attention(attn_launch, e->QKV, e->CTX, M, L, c.heads, e->kbias, varlen ? row_lo : nullptr,
+                           varlen ? row_hi : nullptr, varlen ? tile_kv : nullptr))) return rc;
   for (int l = 0; l < c.n_layer; ++l) {
     const LayerDev& d = e->layers[l];
     uint16_t* X_in = ts ? ts->x(l) : e->X;
@@ -796,7 +856,10 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
     uint16_t* FF = ts ? ts->at(l, ts->lo.ff) : e->FF;
     uint16_t* T2 = ts ? ts->at(l, ts->lo.t2) : e->T;
     uint16_t* X_out = ts ? ts->x(l + 1) : e->X;
-    if (ts && (rc = make_attention(attn_launch, QKV, CTX, M, L, c.heads, ts->kbias(), nullptr, nullptr, nullptr))) return rc;
+    if (ts && (rc = make_attention(attn_launch, QKV, CTX, M, L, c.heads, ts->kbias(), varlen ? row_lo : nullptr,
+                                   varlen ? row_hi : nullptr, varlen ? tile_kv : nullptr))) return rc;
+    attn_launch.ap.row_tok = row_tok;
+    attn_launch.ap.seq_L = L;
     if ((rc = linear<FMT>(X_in, H, M, d.wqkv, 3 * H, H, d.bqkv, nullptr, 0, QKV, nullptr, st, ance::kClsGemmQkv))) return rc;
     if (drop_a) {
       attn_launch.ap.drop = dr->cfg(dr->p_attn, drop::kSiteAttn, l);
@@ -812,15 +875,15 @@ int forward_impl(ance_encoder* e, const int32_t* ids_dev, const int32_t* lens_de
     size_t pitch = cls_only ? static_cast<size_t>(L) * H : H;           // row pitch of CTX / X views
     if (cls_only && varlen) {   // the CLS rows sit at seq_row0[b]: gather them into compact [B, H] operands
       ance::ProfScope ps(ance::kClsNorm, st);
-      gather_rows16_by_index_kernel<<<B, 96, 0, st>>>(e->CTX, e->seq_row0, B, H, e->cls_ctx);
-      gather_rows16_by_index_kernel<<<B, 96, 0, st>>>(e->X, e->seq_row0, B, H, e->cls_x);
+      gather_rows16_by_index_kernel<<<B, 96, 0, st>>>(CTX, seq_row0, B, H, cls_ctx);
+      gather_rows16_by_index_kernel<<<B, 96, 0, st>>>(X_in, seq_row0, B, H, cls_x);
       ANCE_CUDA(cudaGetLastError());
       ance::count_launch(2);
-      ctx_a = e->cls_ctx; res_x = e->cls_x; pitch = H;
+      ctx_a = cls_ctx; res_x = cls_x; pitch = H;
     }
-    // dropout sites 2 and 3: row r of the pruned last layer is token r * L
-    const drop::Cfg dc_out = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, cls_only ? L : 1) : drop::Cfg{};
-    const drop::Cfg dc_ffn = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, cls_only ? L : 1) : drop::Cfg{};
+    // dropout sites 2 and 3: row r of the pruned last layer is token r * L; a packed row r is token row_tok[r]
+    const drop::Cfg dc_out = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, cls_only ? L : 1, cls_only ? nullptr : row_tok) : drop::Cfg{};
+    const drop::Cfg dc_ffn = drop_h ? dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, cls_only ? L : 1, cls_only ? nullptr : row_tok) : drop::Cfg{};
     if (drop_h) rc = linear<FMT, true>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch, &dc_out);
     else rc = linear<FMT>(ctx_a, pitch, Mr, d.wo, H, H, d.bo, res_x, 0, T1, nullptr, st, ance::kClsGemmOut, pitch);
     if (rc) return rc;
@@ -1003,8 +1066,9 @@ int to_bf16(const float* a, uint16_t* o, size_t n, cudaStream_t st) {
   return ANCE_OK;
 }
 
-int add_rows(float* dst, size_t dst_row_stride, const float* src, int rows, int H, cudaStream_t st) {
-  bwd::add_rows_kernel<<<ew_grid(static_cast<size_t>(rows) * H), 256, 0, st>>>(dst, dst_row_stride, src, rows, H);
+int add_rows(float* dst, size_t dst_row_stride, const float* src, int rows, int H, cudaStream_t st,
+             const int32_t* dst_rows = nullptr) {
+  bwd::add_rows_kernel<<<ew_grid(static_cast<size_t>(rows) * H), 256, 0, st>>>(dst, dst_row_stride, src, rows, H, dst_rows);
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);
   return ANCE_OK;
@@ -1046,33 +1110,57 @@ int ln_bwd(const void* x, bool in_f32, size_t x_ld, int rows, int H, const float
   return ANCE_OK;
 }
 
-// dc != null: the forward dropped the probabilities with this site (the kDrop kernels)
+// dc != null: the forward dropped the probabilities with this site (the kDrop kernels).  seq_row0 / seq_len != null: a
+// packed plan, every sequence at its own length (L: the longest)
 template <uint32_t FMT>
 int attn_bwd(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, int B, int L,
-             int heads, cudaStream_t st, const drop::Cfg* dc = nullptr) {
+             int heads, cudaStream_t st, const drop::Cfg* dc = nullptr, const int32_t* seq_row0 = nullptr,
+             const int32_t* seq_len = nullptr) {
   const size_t smem = bwd::attn_bwd_smem(L);
   ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
   ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
   ance::ProfScope ps(ance::kClsAttn, st);
-  if (dc) bwd::attn_bwd_kernel<FMT, true><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f, *dc);
-  else bwd::attn_bwd_kernel<FMT><<<dim3(B, heads), 256, smem, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, L, heads, kLog2e / 8.0f, drop::Cfg{});
+  const int c1 = cls_only ? 1 : 0;
+  const float sl = kLog2e / 8.0f;
+  const dim3 grid(B, heads);
+  if (seq_row0) {
+    ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
+    ANCE_CUDA(cudaFuncSetAttribute(bwd::attn_bwd_kernel<FMT, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bwd::attn_bwd_smem(attn::kTile))));
+    if (dc) bwd::attn_bwd_kernel<FMT, true, true><<<grid, 256, smem, st>>>(qkv, kbias, dout, c1, dqkv, L, heads, sl, *dc, seq_row0, seq_len);
+    else bwd::attn_bwd_kernel<FMT, false, true><<<grid, 256, smem, st>>>(qkv, kbias, dout, c1, dqkv, L, heads, sl, drop::Cfg{}, seq_row0, seq_len);
+  } else if (dc) {
+    bwd::attn_bwd_kernel<FMT, true><<<grid, 256, smem, st>>>(qkv, kbias, dout, c1, dqkv, L, heads, sl, *dc);
+  } else {
+    bwd::attn_bwd_kernel<FMT><<<grid, 256, smem, st>>>(qkv, kbias, dout, c1, dqkv, L, heads, sl, drop::Cfg{});
+  }
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(1);
   return ANCE_OK;
 }
 
-// L in {256, 384, 512}: the key-blocked kernels of attn_bwd_long.cuh; stats: bwdl::stats_floats(B, L, heads) fp32
+// L in {256, 384, 512}: the key-blocked kernels of attn_bwd_long.cuh; stats: bwdl::stats_floats(B, L, heads) fp32.
+// seq_row0 / seq_len != null: a packed plan, every sequence at its own length (L: a multiple of 64 >= the longest)
 template <uint32_t FMT>
 int attn_bwd_long(const uint16_t* qkv, const float* kbias, const uint16_t* dout, bool cls_only, float* dqkv, float* stats,
-                  int B, int L, int heads, cudaStream_t st, const drop::Cfg* dc = nullptr) {
+                  int B, int L, int heads, cudaStream_t st, const drop::Cfg* dc = nullptr, const int32_t* seq_row0 = nullptr,
+                  const int32_t* seq_len = nullptr) {
   const dim3 grid(L / bwdl::kBlk, heads, B);
   ance::ProfScope ps(ance::kClsAttn, st);
-  if (dc) {
-    bwdl::dq_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, *dc);
-    bwdl::dkv_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, *dc);
+  const int c1 = cls_only ? 1 : 0;
+  const float sl = kLog2e / 8.0f;
+  const drop::Cfg d = dc ? *dc : drop::Cfg{};
+  if (seq_row0 && dc) {
+    bwdl::dq_kernel<FMT, true, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d, seq_row0, seq_len);
+    bwdl::dkv_kernel<FMT, true, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d, seq_row0, seq_len);
+  } else if (seq_row0) {
+    bwdl::dq_kernel<FMT, false, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d, seq_row0, seq_len);
+    bwdl::dkv_kernel<FMT, false, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d, seq_row0, seq_len);
+  } else if (dc) {
+    bwdl::dq_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d);
+    bwdl::dkv_kernel<FMT, true><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d);
   } else {
-    bwdl::dq_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, drop::Cfg{});
-    bwdl::dkv_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, cls_only ? 1 : 0, dqkv, stats, L, heads, kLog2e / 8.0f, drop::Cfg{});
+    bwdl::dq_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d);
+    bwdl::dkv_kernel<FMT><<<grid, bwdl::kThreads, 0, st>>>(qkv, kbias, dout, c1, dqkv, stats, L, heads, sl, d);
   }
   ANCE_CUDA(cudaGetLastError());
   ance::count_launch(2);
@@ -1086,7 +1174,7 @@ __global__ void __launch_bounds__(256) dropout_mask_rows_kernel(const float* src
   const size_t n = static_cast<size_t>(rows) * groups;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int r = static_cast<int>(i / groups), g = static_cast<int>(i % groups);
-    const uint4 w = drop::hidden_bits(c, static_cast<uint32_t>(r) * c.tok_stride, g);
+    const uint4 w = drop::hidden_bits(c, drop::row_token(c, r), g);
     const float4* s = reinterpret_cast<const float4*>(src + static_cast<size_t>(r) * H + g * 8);
     float4* d = reinterpret_cast<float4*>(dst + static_cast<size_t>(r) * H + g * 8);
     const float4 a = s[0], b = s[1];
@@ -1159,13 +1247,14 @@ struct BwdScratch {
   float* attn_stats;   // [B * heads, 3, L]: per-row softmax statistics of the L > 128 attention backward
 };
 
-int ensure_scratch(ance_encoder* e, int M, BwdScratch& s) {
+// M: rows of the layers; stat_tokens: B * L of the attention statistics (M for dense batches)
+int ensure_scratch(ance_encoder* e, int M, BwdScratch& s, size_t stat_tokens) {
   const size_t H = e->cfg.hidden, F = e->cfg.ffn, N = std::max(3 * H, F), Mp = (M + 7) / 8 * 8;
   auto up = [](size_t x) { return (x + 255) / 256 * 256; };
   const size_t part = std::max(static_cast<size_t>(bwd::kLnBwdMaxBlocks) * 3 * H, static_cast<size_t>(bwd::kColsumChunks) * N);
   const size_t sz[11] = {up(M * H * 4), up(M * H * 4), up(M * N * 4), up(M * H * 4), up(part * 4),
                          up(M * N * 2), up(N * Mp * 2), up(N * Mp * 2), up(M * H * 2), up(static_cast<size_t>(M) * 4),
-                         up(bwdl::stats_floats(1, M, e->cfg.heads) * 4)};
+                         up(bwdl::stats_floats(1, static_cast<int>(stat_tokens), e->cfg.heads) * 4)};
   size_t total = 0;
   for (size_t x : sz) total += x;
   if (total > e->bwd_scratch_bytes) {
@@ -1198,18 +1287,23 @@ int wgrad(const uint16_t* dYt, int n_out, const uint16_t* Xt, int k_in, int rows
 
 // dr: the dropout of the forward (null or zero rates: none).  At a hidden site T = m o Y s + R, the residual R gets the
 // LayerNorm's dT and the branch (bias, wgrad, dgrad) m o dT s; the embedding LayerNorm gets m o dX0 s.
+// n_tiles > 0: the forward ran the packed plan kept in the workspace.  Every layer's GEMMs and LayerNorms run over its
+// n_tiles * 128 rows; the attention backward runs per sequence at its own length, and the rows of no sequence (tile
+// fillers, and the padding rows a long sequence gets under align 16) keep a zero dQKV, so they add nothing to any sum.
 template <uint32_t FMT>
 int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws, const ance_encoder_grads* g,
-                  cudaStream_t st, const DropState* dr = nullptr) {
+                  cudaStream_t st, const DropState* dr = nullptr, int n_tiles = 0) {
   const bool drop_h = dr && dr->hidden(), drop_a = dr && dr->attn();
   const ance_encoder_config& c = e->cfg;
-  const int H = c.hidden, F = c.ffn, M = B * L, Mp = (M + 7) / 8 * 8, NL = c.n_layer;
+  const bool packed = n_tiles > 0;
+  const int H = c.hidden, F = c.ffn, M = packed ? n_tiles * attn::kTile : B * L, Mp = (M + 7) / 8 * 8, NL = c.n_layer;
   constexpr int S = src_code<FMT>();
-  TrainSave ts{ws, train_layout(c, B, L), NL};
+  const TrainSave ts = train_save(c, ws, B, L, n_tiles);
+  const int L_long = (L + bwdl::kBlk - 1) / bwdl::kBlk * bwdl::kBlk;   // attention statistics per sequence (packed: any L)
   BwdScratch s;
   int rc;
   if ((rc = ensure_wt<FMT>(e, st))) return rc;
-  if ((rc = ensure_scratch(e, M, s))) return rc;
+  if ((rc = ensure_scratch(e, M, s, static_cast<size_t>(B) * L_long))) return rc;
   const int Bp = (B + 7) / 8 * 8;
   // head: out = LN(X_cls Wh^T + bh) -> s.G = d X_cls [B, H]
   if (c.has_head) {
@@ -1240,7 +1334,7 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t2), false, H, Mr, H, d.ln2g, c.ln_eps, s.G, s.dT, s.part, lg.ln2_g, lg.ln2_b, drop_h ? nullptr : lg.ff2_b, st))) return rc;
     const float* dT2 = s.dT;
     if (drop_h) {
-      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, last ? L : 1), st))) return rc;
+      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteFfnOut, l, last ? L : 1, last ? nullptr : ts.row_tok), st))) return rc;
       if ((rc = colsum(s.dX1, Mr, H, s.part, H, lg.ff2_b, nullptr, nullptr, st))) return rc;
       dT2 = s.dX1;
     }
@@ -1266,19 +1360,21 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     if ((rc = ln_bwd<FMT>(ts.at(l, ts.lo.t1), false, H, Mr, H, d.ln1g, c.ln_eps, s.dX1, s.dT, s.part, lg.ln1_g, lg.ln1_b, drop_h ? nullptr : lg.ao_b, st))) return rc;
     const float* dT1 = s.dT;
     if (drop_h) {   // (s.dX1 was the LayerNorm's last input)
-      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, last ? L : 1), st))) return rc;
+      if ((rc = mask_rows(s.dT, s.dX1, Mr, H, dr->cfg(dr->p_hidden, drop::kSiteAttnOut, l, last ? L : 1, last ? nullptr : ts.row_tok), st))) return rc;
       if ((rc = colsum(s.dX1, Mr, H, s.part, H, lg.ao_b, nullptr, nullptr, st))) return rc;
       dT1 = s.dX1;
     }
     if ((rc = to_bf16(dT1, s.A16, static_cast<size_t>(Mr) * H, st))) return rc;
     if ((rc = transpose_bf16<2>(dT1, H, Mr, H, s.Gt, Mrp, st))) return rc;
-    if ((rc = transpose_bf16<S>(ts.at(l, ts.lo.ctx), last ? static_cast<size_t>(L) * H : H, Mr, H, s.Xt, Mrp, st))) return rc;
+    const uint16_t* ctx_rows = (last && packed) ? ts.cls_ctx : ts.at(l, ts.lo.ctx);   // the out-projection's input rows
+    if ((rc = transpose_bf16<S>(ctx_rows, (last && !packed) ? static_cast<size_t>(L) * H : H, Mr, H, s.Xt, Mrp, st))) return rc;
     if ((rc = wgrad(s.Gt, H, s.Xt, H, Mrp, lg.ao_w, st))) return rc;
     if ((rc = linear<kBF>(s.A16, H, Mr, wt.wo, H, H, nullptr, nullptr, 0, s.dCTX, nullptr, st))) return rc;  // d CTX (bf16)
     // attention -> d QKV [M, 3H]
     const drop::Cfg dca = drop_a ? dr->cfg(dr->p_attn, drop::kSiteAttn, l) : drop::Cfg{};
-    if (L <= attn::kTile) rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st, drop_a ? &dca : nullptr);
-    else rc = attn_bwd_long<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, s.attn_stats, B, L, c.heads, st, drop_a ? &dca : nullptr);
+    if (packed) ANCE_CUDA(cudaMemsetAsync(s.dA, 0, static_cast<size_t>(M) * 3 * H * 4, st));   // rows of no sequence
+    if (L <= attn::kTile) rc = attn_bwd<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, B, L, c.heads, st, drop_a ? &dca : nullptr, ts.seq_row0, ts.seq_len);
+    else rc = attn_bwd_long<FMT>(ts.at(l, ts.lo.qkv), ts.kbias(), s.dCTX, last, s.dA, s.attn_stats, B, L_long, c.heads, st, drop_a ? &dca : nullptr, ts.seq_row0, ts.seq_len);
     if (rc) return rc;
     if ((rc = colsum(s.dA, M, 3 * H, s.part, H, lg.q_b, lg.k_b, lg.v_b, st))) return rc;
     if ((rc = to_bf16(s.dA, s.A16, static_cast<size_t>(M) * 3 * H, st))) return rc;
@@ -1288,26 +1384,30 @@ int backward_impl(ance_encoder* e, int B, int L, const float* d_out, uint8_t* ws
     for (int p = 0; p < 3; ++p)
       if ((rc = wgrad(s.Gt + static_cast<size_t>(p) * H * Mp, H, s.Xt, H, Mp, wq[p], st))) return rc;
     if ((rc = linear<kBF>(s.A16, 3 * H, M, wt.wqkv, H, 3 * H, nullptr, nullptr, 0, nullptr, s.G, st))) return rc;   // d X_in
-    if ((rc = add_rows(s.G, last ? L : 1, s.dT, Mr, H, st))) return rc;   // + residual (the CLS rows in the last layer)
+    if ((rc = add_rows(s.G, last ? L : 1, s.dT, Mr, H, st, (last && packed) ? ts.seq_row0 : nullptr))) return rc;   // + residual (the CLS rows in the last layer)
     if (capture) ANCE_CUDA(capture_g(l, M));
   }
   // embeddings: X0 = LN((word[id] + pos[p]) + type[0])
   {
     ance::ProfScope ps(ance::kClsNorm, st);
+    if (packed) {   // rows the sequences do not fill: a zero LayerNorm input (finite, and their dy is zero)
+      ANCE_CUDA(cudaMemsetAsync(s.dA, 0, static_cast<size_t>(M) * H * 4, st));
+      ANCE_CUDA(cudaMemsetAsync(s.pos, 0, static_cast<size_t>(M) * 4, st));
+    }
     bwd::embed_sum_kernel<<<B, 256, 0, st>>>(ts.ids(), L, H, c.arch == ANCE_ARCH_ROBERTA, c.pad_id, c.vocab, c.max_pos,
-                                             e->word, e->pos, e->type, s.dA, s.pos);
+                                             e->word, e->pos, e->type, s.dA, s.pos, ts.seq_row0, ts.seq_len);
     ANCE_CUDA(cudaGetLastError());
     ance::count_launch(1);
   }
   ANCE_CUDA(cudaMemsetAsync(g->word_emb, 0, static_cast<size_t>(c.vocab) * H * 4, st));
   ANCE_CUDA(cudaMemsetAsync(g->pos_emb, 0, static_cast<size_t>(c.max_pos) * H * 4, st));
   ANCE_CUDA(cudaMemsetAsync(g->type_emb, 0, static_cast<size_t>(c.type_vocab) * H * 4, st));
-  if (drop_h && (rc = mask_rows(s.G, s.G, M, H, dr->cfg(dr->p_hidden, drop::kSiteEmbed, 0), st))) return rc;
+  if (drop_h && (rc = mask_rows(s.G, s.G, M, H, dr->cfg(dr->p_hidden, drop::kSiteEmbed, 0, 1, ts.row_tok), st))) return rc;
   if ((rc = ln_bwd<FMT>(s.dA, true, H, M, H, e->eg, c.ln_eps, s.G, s.dT, s.part, g->emb_ln_g, g->emb_ln_b, g->type_emb, st))) return rc;
   {
     ance::ProfScope ps(ance::kClsNorm, st);
     bwd::embed_scatter_kernel<<<M, 256, 0, st>>>(ts.ids(), s.pos, s.dT, M, H, c.arch == ANCE_ARCH_ROBERTA, c.pad_id, c.vocab,
-                                                 g->word_emb, g->pos_emb);
+                                                 g->word_emb, g->pos_emb, ts.row_tok);
     ANCE_CUDA(cudaGetLastError());
     ance::count_launch(1);
   }
@@ -1445,7 +1545,7 @@ int forward_train_impl(ance_encoder_t e, const int32_t* ids_dev, const int32_t* 
   ANCE_REQUIRE(dev == e->device, "%s: the handle belongs to device %d but device %d is current", fn, e->device, dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const TrainSave ts{reinterpret_cast<uint8_t*>(ws_dev), train_layout(c, B, L), c.n_layer};
-  e->train_shapes[ws_dev] = ance_encoder::TrainRecord{B, L, dr.p_hidden, dr.p_attn, dr.seed};
+  e->train_shapes[ws_dev] = ance_encoder::TrainRecord{B, L, dr.p_hidden, dr.p_attn, dr.seed, 0};
   if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts, &dr);
   return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, mask_dev, B, L, out_dev, st, 0, &ts, &dr);
 }
@@ -1492,8 +1592,8 @@ extern "C" int ance_encoder_backward(ance_encoder_t e, const float* d_out_dev, v
   dr.p_hidden = rec.p_hidden;
   dr.p_attn = rec.p_attn;
   dr.seed = rec.seed;
-  if (e->fmt == tc05::kFmtBF16) return backward_impl<tc05::kFmtBF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr);
-  return backward_impl<tc05::kFmtF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr);
+  if (e->fmt == tc05::kFmtBF16) return backward_impl<tc05::kFmtBF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr, rec.n_tiles);
+  return backward_impl<tc05::kFmtF16>(e, rec.B, rec.L, d_out_dev, ws, g, st, &dr, rec.n_tiles);
 }
 
 extern "C" int ance_encoder_update_weights(ance_encoder_t e, const ance_encoder_weights* w_dev, void* stream) {
@@ -1514,6 +1614,7 @@ namespace {
 
 struct PackPlan {
   std::vector<int32_t> row0;     // [placed] first packed row of each sequence
+  std::vector<int32_t> rows;     // [placed] rows of each sequence: its length, or (long, align 16) up to a multiple of 32
   std::vector<int32_t> lo, hi;   // [n_tiles * 128] own-sequence key range of every packed row (absolute rows)
   std::vector<int2> tile_kv;     // [n_tiles] (first key row, number of 128-key blocks) of the tile's attention items
   int n_tiles = 0;
@@ -1543,8 +1644,9 @@ int pack_chunk(const int32_t* lens, int first, int B, int L, int cap_tiles, int 
   std::vector<int> used;            // rows used per tile
   std::vector<int> head(T + 1, -1); // head[f] = a tile with exactly f free rows (intrusive lists through next[])
   std::vector<int> next;
-  std::vector<int> rows;            // rows computed per placed sequence
+  std::vector<int32_t>& rows = plan.rows;
   plan.row0.clear();
+  rows.clear();
   auto push = [&](int tile) { const int f = T - used[tile]; next[tile] = head[f]; head[f] = tile; };
   int placed = 0, cursor = 0;
   for (int b = first; b < B && placed < max_seqs; ++b) {
@@ -1644,7 +1746,106 @@ int forward_packed_impl(ance_encoder_t e, const int32_t* ids_dev, const int32_t*
   return ANCE_OK;
 }
 
+// row -> dense token map of a plan of the sequences 0 .. of a [B, L] batch: row row0[b] + i is token b L + i for each of
+// the plan's rows of sequence b, and a row of no sequence is -1
+std::vector<int32_t> plan_row_tok(const PackPlan& plan, int L) {
+  std::vector<int32_t> tok(static_cast<size_t>(plan.n_tiles) * attn::kTile, -1);
+  for (size_t b = 0; b < plan.row0.size(); ++b)
+    for (int i = 0; i < plan.rows[b]; ++i) tok[plan.row0[b] + i] = static_cast<int32_t>(b) * L + i;
+  return tok;
+}
+
+// The one plan of a packed training batch at the handle's varlen_align (a training batch is never split: its backward
+// needs the whole plan)
+int plan_train_packed(const ance_encoder* e, const int32_t* lens_host, int B, int L, PackPlan& plan, const char* fn) {
+  ANCE_REQUIRE(lens_host != nullptr, "%s: null lens_host", fn);
+  ANCE_REQUIRE(B > 0 && L > 0, "%s: empty batch", fn);
+  if (L > attn::kTile && L > e->train_max_len) {
+    ance::set_error("%s: L = %d; the backward covers sequences of up to %d tokens on this handle (train_max_len; 128, 256, 384 "
+                    "or 512)", fn, L, e->train_max_len);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  const ance_encoder_config& c = e->cfg;
+  ANCE_REQUIRE(L + (c.arch == ANCE_ARCH_ROBERTA ? c.pad_id + 1 : 0) <= c.max_pos, "%s: L = %d exceeds max_position_embeddings %d", fn, L, c.max_pos);
+  for (int b = 0; b < B; ++b)
+    ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= L, "%s: length %d of sequence %d outside [1, %d]", fn, lens_host[b], b, L);
+  const int placed = pack_chunk(lens_host, 0, B, L, e->max_tokens / attn::kTile, e->max_tokens / 16, e->varlen_align, plan);
+  if (placed < B) {
+    long long real = 0;
+    for (int b = 0; b < B; ++b) real += lens_host[b];
+    ance::set_error("%s: the batch (%d sequences, %lld real tokens) does not fit one plan of max_tokens %d rows (%d sequences "
+                    "placed); a packed training batch is planned whole", fn, B, real, e->max_tokens, placed);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  return ANCE_OK;
+}
+
 }  // namespace
+
+extern "C" int ance_encoder_train_workspace_packed(ance_encoder_t e, const int32_t* lens_host, int B, int L, size_t* bytes) {
+  ANCE_REQUIRE(e != nullptr && bytes != nullptr, "ance_encoder_train_workspace_packed: null argument");
+  PackPlan plan;
+  if (const int rc = plan_train_packed(e, lens_host, B, L, plan, "ance_encoder_train_workspace_packed")) return rc;
+  *bytes = packed_layout(e->cfg, B, L, plan.n_tiles).total;
+  return ANCE_OK;
+}
+
+extern "C" int ance_encoder_forward_train_packed(ance_encoder_t e, const int32_t* ids_dev, const int32_t* lens_dev,
+                                                 const int32_t* lens_host, int B, int L, void* ws_dev, float* out_dev,
+                                                 float p_hidden, float p_attn, uint64_t seed, void* stream) {
+  const char* fn = "ance_encoder_forward_train_packed";
+  ANCE_REQUIRE(e != nullptr, "%s: null handle", fn);
+  ANCE_REQUIRE(ids_dev && lens_dev && out_dev && ws_dev, "%s: null buffer", fn);
+  ANCE_REQUIRE((reinterpret_cast<uintptr_t>(ws_dev) & 255u) == 0, "%s: the workspace must be 256-byte aligned", fn);
+  ANCE_REQUIRE(std::isfinite(p_hidden) && p_hidden >= 0.f && p_hidden < 1.f && std::isfinite(p_attn) && p_attn >= 0.f && p_attn < 1.f,
+               "%s: dropout rates must be finite and in [0, 1) (p_hidden = %g, p_attn = %g)", fn, static_cast<double>(p_hidden),
+               static_cast<double>(p_attn));
+  if (p_attn > 0.f && e->varlen_align != 16) {
+    ance::set_error("%s: attention-probability dropout on a packed plan needs varlen_align = 16 (its masks are counted "
+                    "from each sequence's first key, which align 1 may place at any row)", fn);
+    return ANCE_ERR_UNSUPPORTED;
+  }
+  PackPlan plan;
+  if (const int rc = plan_train_packed(e, lens_host, B, L, plan, fn)) return rc;
+  int dev = -1;
+  ANCE_CUDA(cudaGetDevice(&dev));
+  ANCE_REQUIRE(dev == e->device, "%s: the handle belongs to device %d but device %d is current", fn, e->device, dev);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const TrainSave ts = train_save(e->cfg, reinterpret_cast<uint8_t*>(ws_dev), B, L, plan.n_tiles);
+  const std::vector<int32_t> row_tok = plan_row_tok(plan, L);
+  // (pageable cudaMemcpyAsync stages the host arrays before returning)
+  ANCE_CUDA(cudaMemcpyAsync(ts.seq_row0, plan.row0.data(), static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, st));
+  ANCE_CUDA(cudaMemcpyAsync(ts.seq_len, lens_host, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, st));
+  ANCE_CUDA(cudaMemcpyAsync(ts.row_lo, plan.lo.data(), plan.lo.size() * 4, cudaMemcpyHostToDevice, st));
+  ANCE_CUDA(cudaMemcpyAsync(ts.row_hi, plan.hi.data(), plan.hi.size() * 4, cudaMemcpyHostToDevice, st));
+  ANCE_CUDA(cudaMemcpyAsync(ts.row_tok, row_tok.data(), row_tok.size() * 4, cudaMemcpyHostToDevice, st));
+  ANCE_CUDA(cudaMemcpyAsync(ts.tile_kv, plan.tile_kv.data(), plan.tile_kv.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+  DropState dr;
+  dr.p_hidden = p_hidden;
+  dr.p_attn = p_attn;
+  dr.seed = seed;
+  e->train_shapes[ws_dev] = ance_encoder::TrainRecord{B, L, p_hidden, p_attn, seed, plan.n_tiles};
+  if (e->fmt == tc05::kFmtBF16) return forward_impl<tc05::kFmtBF16>(e, ids_dev, lens_dev, nullptr, B, L, out_dev, st, plan.n_tiles, &ts, &dr);
+  return forward_impl<tc05::kFmtF16>(e, ids_dev, lens_dev, nullptr, B, L, out_dev, st, plan.n_tiles, &ts, &dr);
+}
+
+// host-only: the packed training plan's rows (tests) — first rows and the row -> token map of the FIRST chunk
+extern "C" int ance_dbg_pack_rows(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
+                                  int32_t* row_tok_out, int* n_placed, int* n_tiles) {
+  ANCE_REQUIRE(lens_host && row0_out && row_tok_out && n_placed && n_tiles && B > 0, "ance_dbg_pack_rows: bad arguments");
+  ANCE_REQUIRE(L > 0 && L <= 512 && max_tokens >= (L + attn::kTile - 1) / attn::kTile * attn::kTile,
+               "ance_dbg_pack_rows: need 0 < L <= 512 and max_tokens >= L rounded up to 128 (L = %d, max_tokens = %d)", L, max_tokens);
+  ANCE_REQUIRE(align == 1 || align == 16, "ance_dbg_pack_rows: align must be 1 or 16");
+  for (int b = 0; b < B; ++b) ANCE_REQUIRE(lens_host[b] >= 1 && lens_host[b] <= L, "ance_dbg_pack_rows: length %d outside [1, %d]", lens_host[b], L);
+  PackPlan plan;
+  const int mt = max_tokens / attn::kTile * attn::kTile;
+  *n_placed = pack_chunk(lens_host, 0, B, L, mt / attn::kTile, mt / 16, align, plan);
+  *n_tiles = plan.n_tiles;
+  memcpy(row0_out, plan.row0.data(), plan.row0.size() * 4);
+  const std::vector<int32_t> tok = plan_row_tok(plan, L);
+  memcpy(row_tok_out, tok.data(), tok.size() * 4);
+  return ANCE_OK;
+}
 
 // host-only view of the tile packing (tests): plans the FIRST chunk of lens[0..B) for a handle of `max_tokens`
 extern "C" int ance_dbg_pack_varlen(const int32_t* lens_host, int B, int max_tokens, int align, int32_t* row0_out,
@@ -1950,6 +2151,41 @@ extern "C" int ance_dbg_attention_backward_dropout(int fmt, const void* qkv_dev,
   ANCE_CUDA(cudaMallocAsync(&stats, bwdl::stats_floats(B, L, heads) * 4, st));
   const int rc = bf ? attn_bwd_long<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st, &dc)
                     : attn_bwd_long<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L, heads, st, &dc);
+  ANCE_CUDA(cudaFreeAsync(stats, st));
+  return rc;
+}
+
+extern "C" int ance_dbg_attention_backward_packed(int fmt, const void* qkv_dev, const float* kbias_dev,
+                                                  const void* dout_bf16_dev, int cls_only, int B, int L, int heads,
+                                                  const int32_t* seq_row0_dev, const int32_t* seq_len_dev, int n_rows,
+                                                  float p_attn, uint64_t seed, int layer, float* dqkv_dev, void* stream) {
+  const char* fn = "ance_dbg_attention_backward_packed";
+  ANCE_REQUIRE(fmt == ANCE_FMT_FP16 || fmt == ANCE_FMT_BF16, "%s: unknown operand format %d", fn, fmt);
+  ANCE_REQUIRE(qkv_dev && kbias_dev && dout_bf16_dev && dqkv_dev && seq_row0_dev && seq_len_dev, "%s: null buffer", fn);
+  ANCE_REQUIRE(aligned16(qkv_dev) && aligned16(dout_bf16_dev) && aligned16(dqkv_dev), "%s: qkv, dout and dqkv must be 16-byte aligned", fn);
+  ANCE_REQUIRE(heads >= 1 && heads <= 16, "%s: heads = %d outside [1, 16]", fn, heads);
+  ANCE_REQUIRE(B > 0 && L > 0 && L <= 512 && n_rows > 0, "%s: need B > 0, 0 < L <= 512 and n_rows > 0 (B = %d, L = %d, n_rows = %d)", fn, B, L, n_rows);
+  ANCE_REQUIRE(std::isfinite(p_attn) && p_attn >= 0.f && p_attn < 1.f && layer >= 0, "%s: need 0 <= p_attn < 1 and layer >= 0", fn);
+  if (const int rc = require_sm90(nullptr)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const auto* qkv = reinterpret_cast<const uint16_t*>(qkv_dev);
+  const auto* dout = reinterpret_cast<const uint16_t*>(dout_bf16_dev);
+  DropState dr;
+  dr.p_attn = p_attn;
+  dr.seed = seed;
+  const drop::Cfg dc = dr.cfg(p_attn, drop::kSiteAttn, layer);
+  const drop::Cfg* dcp = p_attn > 0.f ? &dc : nullptr;
+  const bool bf = fmt == ANCE_FMT_BF16;
+  // as backward_impl: dQKV zeroed, then the per-sequence launch
+  ANCE_CUDA(cudaMemsetAsync(dqkv_dev, 0, static_cast<size_t>(n_rows) * 3 * heads * attn::kDh * 4, st));
+  if (L <= attn::kTile)
+    return bf ? attn_bwd<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st, dcp, seq_row0_dev, seq_len_dev)
+              : attn_bwd<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, B, L, heads, st, dcp, seq_row0_dev, seq_len_dev);
+  const int L_long = (L + bwdl::kBlk - 1) / bwdl::kBlk * bwdl::kBlk;
+  float* stats = nullptr;
+  ANCE_CUDA(cudaMallocAsync(&stats, bwdl::stats_floats(B, L_long, heads) * 4, st));
+  const int rc = bf ? attn_bwd_long<tc05::kFmtBF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L_long, heads, st, dcp, seq_row0_dev, seq_len_dev)
+                    : attn_bwd_long<tc05::kFmtF16>(qkv, kbias_dev, dout, cls_only != 0, dqkv_dev, stats, B, L_long, heads, st, dcp, seq_row0_dev, seq_len_dev);
   ANCE_CUDA(cudaFreeAsync(stats, st));
   return rc;
 }

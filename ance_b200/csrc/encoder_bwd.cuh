@@ -32,6 +32,8 @@ __device__ __forceinline__ uint16_t float_to_bf16(float f) { return __bfloat16_a
 // P [L][L + 1], later overwritten by dS / 8.  All products are fp32 FMAs on the CUDA cores.
 // dout: bf16 [B*L, H]; with cls_only only token 0 of each sequence has an upstream gradient and dout is [B, H] (the pruned
 // last layer).  dqkv: fp32 [B*L, 3H] (Q | K | V, head-major inside each), every element of the sequence's rows written.
+// Packed row plans (kSeq: seq_row0 / seq_len): sequence b occupies the rows seq_row0[b] .. + seq_len[b] and runs at its
+// own length (its keys are exactly its tokens; the plan's kbias is zero); only those rows of dqkv are written.
 // ------------------------------------------------------------------------------------------------
 constexpr int kAttnPitch = 65;
 inline size_t attn_bwd_smem(int L) { return (static_cast<size_t>(4) * L * kAttnPitch + static_cast<size_t>(L) * (L + 1)) * 4; }
@@ -39,21 +41,23 @@ inline size_t attn_bwd_smem(int L) { return (static_cast<size_t>(4) * L * kAttnP
 // kDrop: the forward dropped probabilities with the mask m of site 1 and scale s (dropout.cuh): P~ = m o P s,
 // dP = m o (dO V^T) s, dV = P~^T dO, D = sum_j P dP, dS = P o (dP - D).  The mask is generated once, with P, and kept as
 // the sign bit of P's shared-memory entry (P >= 0; a dropped P is stored negated, -0 for 0).
-template <uint32_t FMT, bool kDrop = false>
+template <uint32_t FMT, bool kDrop = false, bool kSeq = false>
 __global__ void __launch_bounds__(256) attn_bwd_kernel(const uint16_t* __restrict__ qkv, const float* __restrict__ kbias,
                                                        const uint16_t* __restrict__ dout, int cls_only,
                                                        float* __restrict__ dqkv, int L, int heads, float scale_log2,
-                                                       const drop::Cfg dc) {
+                                                       const drop::Cfg dc, const int32_t* __restrict__ seq_row0 = nullptr,
+                                                       const int32_t* __restrict__ seq_len = nullptr) {
   using A16 = act16::Act<FMT>;
   extern __shared__ float sm[];
   const int b = blockIdx.x, h = blockIdx.y, H = heads * 64;
+  if constexpr (kSeq) L = seq_len[b];
   const int PP = L + 1;
   float* sQ = sm;
   float* sK = sQ + L * kAttnPitch;
   float* sV = sK + L * kAttnPitch;
   float* sO = sV + L * kAttnPitch;   // dO
   float* sP = sO + L * kAttnPitch;
-  const size_t tok0 = static_cast<size_t>(b) * L;
+  const size_t tok0 = kSeq ? static_cast<size_t>(seq_row0[b]) : static_cast<size_t>(b) * L;
   for (int i = threadIdx.x; i < L * 64; i += blockDim.x) {
     const int r = i >> 6, d = i & 63;
     const uint16_t* row = qkv + (tok0 + r) * 3 * H + h * 64 + d;
@@ -390,24 +394,28 @@ __global__ void __launch_bounds__(256) refresh_kernel(const RefreshPiece* __rest
   }
 }
 
-// dst[r * dst_row_stride] += src[r]   (rows of H fp32)
-__global__ void add_rows_kernel(float* __restrict__ dst, size_t dst_row_stride, const float* __restrict__ src, int rows, int H) {
+// dst[r * dst_row_stride] += src[r], or dst[dst_rows[r]] += src[r]   (rows of H fp32)
+__global__ void add_rows_kernel(float* __restrict__ dst, size_t dst_row_stride, const float* __restrict__ src, int rows, int H,
+                                const int32_t* __restrict__ dst_rows = nullptr) {
   const size_t n = static_cast<size_t>(rows) * H;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const size_t r = i / H, c = i % H;
-    dst[r * dst_row_stride * H + c] += src[i];
+    dst[(dst_rows ? static_cast<size_t>(dst_rows[r]) : r * dst_row_stride) * H + c] += src[i];
   }
 }
 
 // The embedding LayerNorm's input E = (word[id] + pos[p]) + type[0] (fp32, the forward's association) and the position id
 // of every token of sequence b = blockIdx.x; positions follow the forward's rule (RoBERTa: cumsum of non-pad tokens + pad,
 // pad tokens at pad; BERT: 0 .. L-1).  Ids / positions out of range are clamped as in the forward.  L <= kEmbedMaxL: the
-// scan runs over chunks of 256 tokens, carrying the count of the chunks before.
+// scan runs over chunks of 256 tokens, carrying the count of the chunks before.  Packed row plans (seq_row0 / seq_len not
+// null): ids_all is still the dense [B, L] batch, and token i < seq_len[b] of sequence b goes to row seq_row0[b] + i.
 constexpr int kEmbedMaxL = 512;
 __global__ void __launch_bounds__(256) embed_sum_kernel(const int32_t* __restrict__ ids_all, int L, int H, int roberta,
                                                         int pad_id, int vocab, int max_pos, const float* __restrict__ word,
                                                         const float* __restrict__ pos, const float* __restrict__ type,
-                                                        float* __restrict__ E, int32_t* __restrict__ pos_out) {
+                                                        float* __restrict__ E, int32_t* __restrict__ pos_out,
+                                                        const int32_t* __restrict__ seq_row0 = nullptr,
+                                                        const int32_t* __restrict__ seq_len = nullptr) {
   __shared__ int s_pos[kEmbedMaxL];
   __shared__ int s_warp_cnt[8];
   const int b = blockIdx.x;
@@ -429,8 +437,9 @@ __global__ void __launch_bounds__(256) embed_sum_kernel(const int32_t* __restric
     carry = total;
     __syncthreads();
   }
-  for (int t = warp; t < L; t += 8) {
-    const size_t tok = static_cast<size_t>(b) * L + t;
+  const int t_end = seq_len ? seq_len[b] : L;
+  for (int t = warp; t < t_end; t += 8) {
+    const size_t tok = (seq_row0 ? static_cast<size_t>(seq_row0[b]) : static_cast<size_t>(b) * L) + t;
     const int id = min(max(ids[t], 0), vocab - 1);
     const int ps = min(s_pos[t], max_pos - 1);
     if (lane == 0) pos_out[tok] = ps;
@@ -441,13 +450,17 @@ __global__ void __launch_bounds__(256) embed_sum_kernel(const int32_t* __restric
 
 // word / position gradient rows += dE of every token (fp32 atomics: the order of the additions into a row that several
 // tokens share is not deterministic).  The padding row of each table that the reference declares with padding_idx gets
-// no gradient: word row pad_id always, position row pad_id for RoBERTa.
+// no gradient: word row pad_id always, position row pad_id for RoBERTa.  Packed row plans (row_tok not null): row r is
+// token row_tok[r] of the dense ids, and a row of no sequence (-1) adds nothing.
 __global__ void embed_scatter_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ pos_ids,
                                      const float* __restrict__ dE, int M, int H, int roberta, int pad_id, int vocab,
-                                     float* __restrict__ dword, float* __restrict__ dpos) {
+                                     float* __restrict__ dword, float* __restrict__ dpos,
+                                     const int32_t* __restrict__ row_tok = nullptr) {
   const int tok = blockIdx.x;
   if (tok >= M) return;
-  const int raw = ids[tok];
+  const int dense_tok = row_tok ? row_tok[tok] : tok;
+  if (dense_tok < 0) return;
+  const int raw = ids[dense_tok];
   const int id = min(max(raw, 0), vocab - 1), ps = pos_ids[tok];
   const bool w_ok = raw != pad_id, p_ok = !(roberta && ps == pad_id);
   for (int c = threadIdx.x; c < H; c += blockDim.x) {

@@ -95,7 +95,7 @@ __device__ __forceinline__ void gelu_logistic2(float& x0, float& x1) {
 
 // FMT: 16-bit format of the OUTPUT and of the residual (act16.cuh); the operand format of the GEMM itself is the
 // FMT parameter of gemm::launch.  kDrop: dropout between the bias (and activation) and the residual, in fp32 before the
-// one rounding: C = m o (A W^T + bias) / (1 - p) + R, the mask of output row r being that of token r * drop.tok_stride.
+// one rounding: C = m o (A W^T + bias) / (1 - p) + R, the mask of output row r being that of token drop::row_token(r).
 template <int BN, int EPI_WARPS, uint32_t FMT = tc05::kFmtBF16, bool kDrop = false>
 struct EpStore {
   using A16 = act16::Act<FMT>;
@@ -164,7 +164,7 @@ struct EpStore {
     }
     if constexpr (kDrop) {
       if (row_ok) {
-        const uint32_t t = static_cast<uint32_t>(row) * static_cast<uint32_t>(p.drop.tok_stride);
+        const uint32_t t = drop::row_token(p.drop, row);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const uint4 w = drop::hidden_bits(p.drop, t, static_cast<uint32_t>(col0 >> 3) + k);

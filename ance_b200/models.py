@@ -164,6 +164,7 @@ class _CudaEncoder:
                                      f"weight {tuple(lin.weight.shape)}")
         w, lw = _fill(_lib.EncoderWeights, _lib.LayerWeights, _param_groups(backbone, head), fp)
         self.hidden_size = H
+        self.pad_id = int(pad_id)
         self.max_tokens = int(max_tokens)
         h = C.c_void_p()
         with torch.cuda.device(device):
@@ -254,6 +255,25 @@ class _CudaEncoder:
                                                                        _lib.current_stream()))
         return out, ws
 
+    def forward_train_packed(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: torch.Tensor,
+                             dropout: Optional[tuple] = None, align: int = 16):
+        """forward_train() of a [B, L] batch whose row b is the non-empty prefix of lens[b] tokens, computing the real
+        tokens only (ance_encoder_forward_train_packed): lens int32 [B] on the device and lens_host the same on the host;
+        align 16 gives forward_train's output bit for bit, 1 packs densest.  -> (out fp32 [B, H], workspace tensor)."""
+        B, L = ids.shape
+        lens_host = lens_host.to(torch.int32).contiguous()
+        self.set_param("varlen_align", align)
+        n = C.c_size_t()
+        _lib.check(self.lib.ance_encoder_train_workspace_packed(self.h, lens_host.data_ptr(), B, L, C.byref(n)))
+        ws = torch.empty(n.value, dtype=torch.uint8, device=ids.device)
+        out = torch.empty((B, self.hidden_size), dtype=torch.float32, device=ids.device)
+        p_hidden, p_attn, seed = dropout if dropout is not None else (0.0, 0.0, 0)
+        with torch.cuda.device(ids.device):
+            _lib.check(self.lib.ance_encoder_forward_train_packed(
+                self.h, ids.data_ptr(), lens.data_ptr(), lens_host.data_ptr(), B, L, ws.data_ptr(), out.data_ptr(),
+                float(p_hidden), float(p_attn), int(seed), _lib.current_stream()))
+        return out, ws
+
     def backward(self, d_out: torch.Tensor, ws: torch.Tensor, grads) -> None:
         """Gradients of sum(d_out * out) for the forward_train that filled `ws`, written into `grads` (fp32 tensors
         grouped as _param_groups)."""
@@ -264,12 +284,16 @@ class _CudaEncoder:
 
 
 class _TrainableEncode(torch.autograd.Function):
-    """Embeddings [B, H] of a dense batch as a function of the encoder's parameters (the `params` inputs, in
-    _param_groups order), so that their .grad accumulates and DDP's hooks fire."""
+    """Embeddings [B, H] of a batch as a function of the encoder's parameters (the `params` inputs, in _param_groups
+    order), so that their .grad accumulates and DDP's hooks fire.  packed = (lens_host, align): the packed forward of
+    prefix rows of lens (forward_train_packed); None: the dense forward."""
 
     @staticmethod
-    def forward(ctx, enc, n_layer, ids, lens, mask, dropout, *params):
-        out, ws = enc.forward_train(ids, lens, mask, dropout)
+    def forward(ctx, enc, n_layer, ids, lens, mask, dropout, packed, *params):
+        if packed is None:
+            out, ws = enc.forward_train(ids, lens, mask, dropout)
+        else:
+            out, ws = enc.forward_train_packed(ids, lens, packed[0], dropout, packed[1])
         ctx.enc, ctx.ws, ctx.n_layer = enc, ws, n_layer
         ctx.shapes = [p.shape for p in params]
         return out
@@ -282,7 +306,7 @@ class _TrainableEncode(torch.autograd.Function):
         n = ctx.n_layer
         groups = (flat[:5], [flat[5 + 16 * i:5 + 16 * (i + 1)] for i in range(n)], flat[5 + 16 * n:])
         ctx.enc.backward(d_out.float().contiguous(), ctx.ws, groups)
-        return (None, None, None, None, None, None, *flat)
+        return (None, None, None, None, None, None, None, *flat)
 
 
 def _forward_varlen(self, ids: torch.Tensor, lens: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
@@ -339,12 +363,13 @@ class _B200Encoder(nn.Module):
     _trainable = False
     _train_max_len = 128
     _dropout = (0.0, 0.0)   # (hidden, attention-probability) rates of the trainable forward in train() mode
+    _packed = False         # set_trainable(..., packed=True): prefix-mask batches train through the packed forward
 
     def _default_dropout(self) -> tuple:
         """dropout=True: the checkpoint config's hidden_dropout_prob / attention_probs_dropout_prob."""
         return (float(self.config.hidden_dropout_prob), float(self.config.attention_probs_dropout_prob))
 
-    def set_trainable(self, on: bool = True, max_len: int = 128, dropout=False):
+    def set_trainable(self, on: bool = True, max_len: int = 128, dropout=False, packed: bool = False):
         """Opt in to gradients: while torch grad mode is on, query_emb / body_emb / encode_lens (dense batches of up to
         `max_len` tokens per sequence or MaxP chunk: 8, 16, 32, 64 or 128, or a multiple of 128 up to max_len) and the
         triplet forward() return tensors whose backward runs the encoder's backward kernels; the other encode paths raise
@@ -354,7 +379,17 @@ class _B200Encoder(nn.Module):
         rates of the config (RoBERTa: hidden_dropout_prob / attention_probs_dropout_prob; the DPR BiEncoder: 0.1 / 0.1);
         a float sets both rates.  Dropout is applied only on the gradient path and only while the module is in train()
         mode (from_pretrained ends in eval()); each encode draws its mask seed from torch's default CPU generator, so
-        torch.manual_seed reproduces a step."""
+        torch.manual_seed reproduces a step.
+
+        packed: False (default) trains the padded [B, L] batch.  True computes the real tokens only: an encode whose rows
+        each have a non-empty prefix mask (as the token caches produce) runs as ONE packed training forward and backward
+        (varlen_align 16: the same embeddings, dropout masks and loss as the dense path; gradients equal up to fp32
+        summation order), with its lengths from one device-to-host copy.  Other encodes are split: the prefix rows go
+        packed, rows of no real token whose ids are all padding share one dense encode of such a row (MaxP's empty
+        chunks), any other row takes the dense path.  Such a split encode gives the dense path's values without dropout;
+        with dropout each part draws its own seed and numbers its sequences from 0, and the empty chunks share one mask,
+        so its masks are not the padded batch's.  L may be any length up to max_len, and encode_lens_packed becomes
+        trainable.  A batch must fit one plan of max_tokens rows."""
         if max_len not in (128, 256, 384, 512):
             raise ValueError(f"max_len must be 128, 256, 384 or 512, got {max_len!r}")
         if dropout is True:
@@ -368,6 +403,7 @@ class _B200Encoder(nn.Module):
         self._trainable = bool(on)
         self._train_max_len = int(max_len)
         self._dropout = rates
+        self._packed = bool(packed)
         return self
 
     def _train_dropout(self) -> Optional[tuple]:
@@ -386,28 +422,86 @@ class _B200Encoder(nn.Module):
                                  f"{self._train_max_len} tokens through query_emb / body_emb / encode_lens (or run this "
                                  "under torch.no_grad())")
 
-    def _train_emb(self, enc, backbone, head, ids, lens, mask):
+    def _train_emb(self, enc, backbone, head, ids, lens, mask, align: int = 16):
         B, L = ids.shape
         max_len = self._train_max_len
         if L > max_len:
             raise _lib.AnceError(f"inputs of {L} tokens have no backward: the trainable encoder covers up to max_len = "
                                  f"{max_len} tokens (set_trainable(True, max_len=...) takes 128, 256, 384 or 512; or run "
                                  "longer inputs under torch.no_grad())")
+        if self._packed:
+            return self._train_emb_routed(enc, backbone, head, ids, lens, mask, align)
+        return self._train_emb_dense(enc, backbone, head, ids, lens, mask)
+
+    def _train_params(self, enc, backbone, head):
+        """Refresh the handle from the parameters; -> (number of layers, the parameters in _param_groups order)."""
+        # The device weights are refreshed from the parameters before every training forward, whatever their `_version`
+        # says: optimizers that write through `p.data` (the reference trainer's Lamb, transformers' AdamW) do not bump it.
+        if not enc.update_weights(backbone, head):
+            raise _lib.AnceError("a trainable encoder needs contiguous fp32 parameters on the inputs' device")
+        max_len = self._train_max_len
+        if getattr(enc, "_train_max_len", 128) != max_len:
+            enc.set_param("train_max_len", max_len)
+            enc._train_max_len = max_len
+        embs, layers, hd = _param_groups(backbone, head)
+        return len(layers), embs + [t for l in layers for t in l] + hd
+
+    def _train_emb_routed(self, enc, backbone, head, ids, lens, mask, align):
+        """packed=True: prefix rows through the packed forward, all-padding rows through one dense encode of such a row,
+        the rest through the dense path; one device-to-host copy of the lengths (and prefix flags)."""
+        B, L = ids.shape
+        dev = ids.device
+        if lens is None:
+            m = mask != 0
+            lens_d = m.sum(dim=1, dtype=torch.int32)
+            prefix = (m == (torch.arange(L, device=dev)[None, :] < lens_d[:, None])).all(dim=1)
+            lh, pre = torch.stack([lens_d, prefix.to(torch.int32)]).cpu()
+        else:
+            lh = lens.cpu()
+            pre = torch.ones(B, dtype=torch.int32)
+        ok = (pre != 0) & (lh >= 1) & (lh <= L)
+        tp = n_layer, params = self._train_params(enc, backbone, head)   # one weight refresh for all the sub-encodes
+        if bool(ok.all()):
+            lh32 = lh.to(torch.int32)
+            return _TrainableEncode.apply(enc, n_layer, ids, lh32.to(dev), None, self._train_dropout(), (lh32, align),
+                                          *params)
+        parts = []
+        sel = torch.nonzero(ok).flatten()
+        if sel.numel():
+            lh32 = lh[sel].to(torch.int32)
+            sd = sel.to(dev)
+            parts.append((sel, _TrainableEncode.apply(enc, n_layer, ids[sd].contiguous(), lh32.to(dev), None,
+                                                      self._train_dropout(), (lh32, align), *params)))
+        rest = torch.nonzero(~ok).flatten()
+        rd = rest.to(dev)
+        allpad = (lh[rest] == 0) & (ids[rd] == enc.pad_id).all(dim=1).cpu()
+        pad_rows, other = rest[allpad], rest[~allpad]
+        if pad_rows.numel():   # every all-padding row has the same embedding: one encode, broadcast
+            one = ids[rd[allpad.to(dev)][:1]].contiguous()
+            z = None if lens is None else torch.zeros(1, dtype=lens.dtype, device=dev)
+            zm = None if mask is None else torch.zeros((1, L), dtype=mask.dtype, device=dev)
+            emb = self._train_emb_dense(enc, backbone, head, one, z, zm, tp)
+            parts.append((pad_rows, emb.expand(pad_rows.numel(), emb.shape[1])))
+        if other.numel():
+            od = other.to(dev)
+            parts.append((other, self._train_emb_dense(enc, backbone, head, ids[od].contiguous(),
+                                                       None if lens is None else lens[od].contiguous(),
+                                                       None if mask is None else mask[od].contiguous(), tp)))
+        order = torch.cat([p[0] for p in parts])
+        inv = torch.empty_like(order)
+        inv[order] = torch.arange(B)
+        return torch.cat([p[1] for p in parts])[inv.to(dev)]
+
+    def _train_emb_dense(self, enc, backbone, head, ids, lens, mask, tp=None):
+        """tp: (n_layer, params) of a _train_params call already made for this encode (else it is made here)."""
+        B, L = ids.shape
         if L > 128 and L % 128:
             raise _lib.AnceError(f"inputs of {L} tokens have no backward: above 128 tokens the trainable encoder takes "
                                  "multiples of 128 (pad the batch to 256, 384 or 512)")
         if B * L > enc.max_tokens:
             raise _lib.AnceError(f"a trainable batch of {B} x {L} tokens exceeds max_tokens {enc.max_tokens}")
-        # The device weights are refreshed from the parameters before every training forward, whatever their `_version`
-        # says: optimizers that write through `p.data` (the reference trainer's Lamb, transformers' AdamW) do not bump it.
-        if not enc.update_weights(backbone, head):
-            raise _lib.AnceError("a trainable encoder needs contiguous fp32 parameters on the inputs' device")
-        if getattr(enc, "_train_max_len", 128) != max_len:
-            enc.set_param("train_max_len", max_len)
-            enc._train_max_len = max_len
-        embs, layers, hd = _param_groups(backbone, head)
-        params = embs + [t for l in layers for t in l] + hd
-        return _TrainableEncode.apply(enc, len(layers), ids, lens, mask, self._train_dropout(), *params)
+        n_layer, params = tp if tp is not None else self._train_params(enc, backbone, head)
+        return _TrainableEncode.apply(enc, n_layer, ids, lens, mask, self._train_dropout(), None, *params)
 
     def _enc_for(self, name, backbone, arch, heads, pad_id, head, device) -> _CudaEncoder:
         if device.type != "cuda":
@@ -562,13 +656,19 @@ class RobertaDot_NLL_LN(_B200Encoder):
                                                             align=align)
 
     def encode_lens_packed(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, lens_host: Optional[torch.Tensor] = None,
-                           out: Optional[torch.Tensor] = None, align: int = 1) -> torch.Tensor:
+                           out: Optional[torch.Tensor] = None, align: Optional[int] = None) -> torch.Tensor:
         """encode_lens at the cost of the REAL tokens only, for any L <= 512 (lengths in [1, L]).  align = 16: bit-identical
         to encode_lens at the same L, whatever else is in the batch; align = 1: densest packing, equal up to fp32
-        summation order.  L <= 128 is encode_lens_varlen."""
+        summation order.  align None: 1 for inference, 16 on the trainable path (set_trainable(..., packed=True) with
+        grad enabled), where attention dropout needs it.  L <= 128 is encode_lens_varlen."""
+        if self._grad_path() and self._packed and out is None:
+            if lens_host is not None:
+                raise _lib.AnceError("the trainable encode_lens_packed reads the lengths itself: pass lens_host=None")
+            return self._train_emb(self._encoder(ids_i32.device), self.roberta, (self.embeddingHead, self.norm),
+                                   ids_i32.contiguous(), lens_i32.contiguous(), None, 16 if align is None else align)
         self._refuse_grad("encode_lens_packed")
         return self._encoder(ids_i32.device).forward_packed(ids_i32.contiguous(), lens_i32.contiguous(), lens_host, out=out,
-                                                            align=align)
+                                                            align=1 if align is None else align)
 
     def encode_lens_bucketed(self, ids_i32: torch.Tensor, lens_i32: torch.Tensor, min_bucket: int = 16,
                              out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -710,13 +810,14 @@ class BiEncoder(_B200Encoder):
         self.ctx_model = _backbone(d.vocab_size, d.hidden_size, d.num_hidden_layers, d.intermediate_size,
                                    d.max_position_embeddings, d.type_vocab_size, d.pad_token_id, d.layer_norm_eps)
 
-    def set_trainable(self, on: bool = True, max_len: Optional[int] = None, dropout=False):
+    def set_trainable(self, on: bool = True, max_len: Optional[int] = None, dropout=False, packed: bool = False):
         """As _B200Encoder.set_trainable for both BERT encoders; training needs an explicit max_len (DPR's inputs are 256
-        tokens: set_trainable(True, max_len=256)).  dropout=True is HFBertEncoder.init_encoder's default rate, 0.1."""
+        tokens: set_trainable(True, max_len=256)).  dropout=True is HFBertEncoder.init_encoder's default rate, 0.1.
+        packed=True: prefix-mask rows (mask input_ids != 0) train through the packed forward."""
         if on and max_len is None:
             raise NotImplementedError("the DPR BiEncoder trains on 256-token inputs: call set_trainable(True, max_len=256) "
                                       "(or 128 / 384 / 512 for other input lengths)")
-        return super().set_trainable(on, 128 if max_len is None else max_len, dropout)
+        return super().set_trainable(on, 128 if max_len is None else max_len, dropout, packed)
 
     def _default_dropout(self) -> tuple:
         return (0.1, 0.1)   # model/models.py:229-233, init_encoder(dropout=0.1)

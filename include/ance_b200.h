@@ -265,8 +265,24 @@ int ance_encoder_forward_train(ance_encoder_t enc, const int32_t* ids_dev, const
 int ance_encoder_forward_train_dropout(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev,
                                        const uint8_t* mask_dev, int B, int L, void* ws_dev, float* out_dev, float p_hidden,
                                        float p_attn, uint64_t seed, void* stream);
+/* Packed variable-length training: the training forward of a [B, L] batch whose sequence b is the non-empty prefix of
+ * lens_host[b] tokens, computing the real tokens only.  The batch is planned as ance_encoder_forward_packed plans it, at the
+ * handle's "varlen_align", as ONE plan: ANCE_ERR_UNSUPPORTED when it needs more than max_tokens rows.  Lengths must lie in
+ * [1, L]; L is any length up to 128, or up to the handle's "train_max_len" (ANCE_ERR_UNSUPPORTED above it).
+ * ance_encoder_train_workspace_packed: the workspace bytes of that plan (its rows' activations, plus the plan and the CLS
+ * rows of the pruned last layer, so that several packed forwards may precede their backwards).
+ * ance_encoder_forward_train_packed: dropout as ance_encoder_forward_train_dropout (rates of 0: none), with the masks of the
+ * dense [B, L] batch (token b L + i), so that with varlen_align 16 out_dev is bit-identical to the dense training forward's
+ * at the same seed.  p_attn > 0 needs varlen_align 16 (ANCE_ERR_UNSUPPORTED otherwise).  ids_dev [B, L] int32 (the
+ * padded batch), lens_host the lengths on the host (the plan and the kernels use them: the workspace keeps their copy),
+ * lens_dev the same lengths on the device.  ance_encoder_backward then runs the
+ * backward of this plan. */
+int ance_encoder_train_workspace_packed(ance_encoder_t enc, const int32_t* lens_host, int B, int L, size_t* bytes);
+int ance_encoder_forward_train_packed(ance_encoder_t enc, const int32_t* ids_dev, const int32_t* lens_dev,
+                                      const int32_t* lens_host, int B, int L, void* ws_dev, float* out_dev, float p_hidden,
+                                      float p_attn, uint64_t seed, void* stream);
 /* Gradients of sum(d_out o out) with respect to every weight, for the forward that filled ws_dev (the weights must not
- * have changed since).  d_out_dev [B, hidden] fp32, 16-byte aligned.  The handle forgets ws_dev once this call is made:
+ * have changed since; dense or packed, as that forward was).  d_out_dev [B, hidden] fp32, 16-byte aligned.  The handle forgets ws_dev once this call is made:
  * a second backward from the same workspace is ANCE_ERR_INVALID.  Backward GEMM operands are bf16 whatever operand_fmt is, with fp32
  * accumulation; residual-stream and weight gradients are fp32.  Weight rows that the reference declares as padding_idx get
  * no gradient (word row pad_id; position row pad_id for RoBERTa).  The word / position gradients are scatter-added with
@@ -311,6 +327,11 @@ int ance_dbg_pack_varlen(const int32_t* lens_host, int B, int max_tokens, int al
  * items.  The three arrays may be null. */
 int ance_dbg_pack_packed(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
                          int32_t* lo_out, int32_t* hi_out, int32_t* tile_kv_out, int* n_placed, int* n_tiles);
+/* Host-only: the rows of that plan as ance_encoder_forward_train_packed keeps them: row0_out[i] as above and
+ * row_tok_out [*n_tiles * 128] = the dense token b L + i that each packed row computes (sequence b = token / L), -1 for a
+ * row of no sequence. */
+int ance_dbg_pack_rows(const int32_t* lens_host, int B, int L, int max_tokens, int align, int32_t* row0_out,
+                       int32_t* row_tok_out, int* n_placed, int* n_tiles);
 /* D[M,N] = act(A[M,K] * B[N,K]^T + bias) + R ; A,B 16-bit device arrays in `fmt`; R and the 16-bit output D are bf16
  * whatever `fmt` is; outputs optional; act 0 none, 1 GELU (erfc form), 2 GELU (logistic form).
  * variant (N tile BN, CTA cluster CG, operand stages): 0 = BN 128 CG 1 4 stages, 1 = BN 128 CG 1 3 stages,
@@ -377,6 +398,15 @@ int ance_dbg_dropout_bits(uint64_t seed, uint64_t stream_word, uint64_t first_co
 int ance_dbg_attention_backward_dropout(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
                                         int cls_only, int B, int L, int heads, float p_attn, uint64_t seed, int layer,
                                         float* dqkv_dev, void* stream);
+/* The packed training backward's attention launch (ance_encoder_backward of a packed plan): sequence b occupies rows
+ * seq_row0_dev[b] .. + seq_len_dev[b] of qkv [n_rows, 3 * 64 heads] (and of dout [n_rows, 64 heads] bf16, or dout [B, 64
+ * heads] with cls_only), each at its own length <= L (<= 128: attn_bwd_kernel; up to 512: the key-blocked kernels).
+ * dqkv_dev [n_rows, 3 * 64 heads] fp32 is zeroed first, as the backward does, so rows of no sequence come back 0.
+ * p_attn > 0 applies the site-1 dropout of `layer` with `seed` (counters: sequence b, query and key in the sequence). */
+int ance_dbg_attention_backward_packed(int fmt, const void* qkv_dev, const float* kbias_dev, const void* dout_bf16_dev,
+                                       int cls_only, int B, int L, int heads, const int32_t* seq_row0_dev,
+                                       const int32_t* seq_len_dev, int n_rows, float p_attn, uint64_t seed, int layer,
+                                       float* dqkv_dev, void* stream);
 /* Host-only: the byte offsets of the workspace ance_encoder_forward_train fills for a [B, L] batch (L <= 128, or a multiple
  * of 128 up to the handle's "train_max_len"), out[15] =
  * ids, kbias, layers, per_layer, x_in, qkv, ctx, t1, x1, u, ff, t2, x_final, head_in, total.  ids [B * L] int32 and kbias
