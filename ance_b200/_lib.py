@@ -115,6 +115,8 @@ SIGNATURES = {
     "ance_encoder_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(EncoderGrads), C.c_void_p]),
     "ance_encoder_update_weights": (C.c_int, [C.c_void_p, C.POINTER(EncoderWeights), C.c_void_p]),
     "ance_encoder_debug_grads": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_lamb_step": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_int, C.c_void_p, C.c_void_p]),
     "ance_profile_enable": (C.c_int, [C.c_int]),
     "ance_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "ance_dbg_pack_varlen": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -213,7 +215,7 @@ def index_state(handle, item: str, out) -> None:
 
 
 PROFILE_CLASSES = ("gemm_head", "attention", "norm_embed", "quantize", "coarse_search", "rescore", "exact",
-                   "gemm_qkv", "gemm_out", "gemm_ffn1", "gemm_ffn2")
+                   "gemm_qkv", "gemm_out", "gemm_ffn1", "gemm_ffn2", "optim")
 
 
 def profile_enable(on: bool = True) -> None:

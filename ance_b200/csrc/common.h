@@ -13,7 +13,8 @@ void count_launch(int n);
 
 // device-time profile by kernel class (see ance_profile_enable in the header)
 enum KernelClass { kClsGemm = 0, kClsAttn = 1, kClsNorm = 2, kClsQuant = 3, kClsCoarse = 4, kClsRescore = 5, kClsExact = 6,
-                   kClsGemmQkv = 7, kClsGemmOut = 8, kClsGemmFfn1 = 9, kClsGemmFfn2 = 10, kNumCls = 12 };
+                   kClsGemmQkv = 7, kClsGemmOut = 8, kClsGemmFfn1 = 9, kClsGemmFfn2 = 10, kClsOptim = 11,
+                   kNumCls = 12 };
 void prof_begin(int cls, cudaStream_t st);
 void prof_end(int cls, cudaStream_t st);
 struct ProfScope {

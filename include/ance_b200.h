@@ -303,10 +303,27 @@ int ance_encoder_update_weights(ance_encoder_t enc, const ance_encoder_weights* 
 int ance_encoder_debug_grads(ance_encoder_t enc, int slot, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * LAMB optimizer step  — replaces utils/lamb.py's Lamb.step (one eager pass per parameter tensor)
+ *   reference: utils/lamb.py:24-100, built at drivers/run_ann.py:81, utils/dpr_utils.py:90, drivers/run_warmup.py:77
+ * One step over n contiguous fp32 device tensors: parameters p_dev[t], gradients g_dev[t], moment states m_dev[t] and
+ * v_dev[t] (all four numel[t] elements, written in place except g), hyperparameters hyper[5 t .. 5 t + 4] = lr, beta1,
+ * beta2, eps, weight_decay of the tensor's group.  With u = m / (sqrt(v) + eps) + weight_decay p (after the moment update,
+ * p before this step's), w = min(||p||, 10), a = ||u||, r = w / a (1 when w or a is 0):
+ *   m <- beta1 m + (1 - beta1) g,  v <- beta2 v + (1 - beta2) g^2,  p <- p - lr (adam ? 1 : r) u
+ * and norms_dev[3 t .. 3 t + 2] = (w, a, r), r before the adam override.  No bias correction.  Three kernels on `stream`
+ * whatever n (one when every numel is 0), no host synchronisation, no float atomics: the same inputs give the same bits.
+ * The host arrays are consumed before the call returns.  Pointers need only 4-byte alignment (views at any offset);
+ * numel may be 0 (then the pointers may be null).  At most 512 tensors and 16 distinct hyperparameter tuples per call
+ * (the table travels as kernel parameters), else ANCE_ERR_UNSUPPORTED; split larger steps into several calls.  Bad
+ * arguments are rejected before anything is enqueued. */
+int ance_lamb_step(int n, float* const* p_dev, const float* const* g_dev, float* const* m_dev, float* const* v_dev,
+                   const int64_t* numel, const double* hyper, int adam, float* norms_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Device-time profile by kernel class (bench.py's roofline numbers): CUDA events recorded around every
  * launch on the launch stream.  Classes: 0 encoder GEMM, 1 attention, 2 LayerNorm/embedding/gather,
  * 3 operand quantisation, 4 coarse search GEMM, 5 exact rescore, 6 exact brute force, 7-10 encoder
- * GEMMs by role (QKV, attention out-proj, FFN up, FFN down; class 0 then holds the head GEMM only).
+ * GEMMs by role (QKV, attention out-proj, FFN up, FFN down; class 0 then holds the head GEMM only), 11 optimizer step.
  * ance_profile_read synchronises the device, returns milliseconds and launch counts per class
  * (arrays of length n <= 12) and optionally resets the accumulators.
  * ------------------------------------------------------------------------------------------------ */
