@@ -152,6 +152,8 @@ SIGNATURES = {
     "ance_dbg_transpose_bf16": (C.c_int, [C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p]),
     "ance_dbg_train_layout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "ance_dbg_train_layout_packed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t),
+                                               C.POINTER(C.c_int)]),
     "ance_dbg_index_state": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
 }
 
@@ -162,6 +164,8 @@ INDEX_STATE_ITEMS = ("mu", "centred", "p16", "pstats", "ndelta", "q16", "qn_hat"
 # ance_dbg_train_layout's fields, in order
 TRAIN_LAYOUT_FIELDS = ("ids", "kbias", "layers", "per_layer", "x_in", "qkv", "ctx", "t1", "x1", "u", "ff", "t2",
                        "x_final", "head_in", "total")
+# ance_dbg_train_layout_packed's fields after TRAIN_LAYOUT_FIELDS, in order
+PACKED_LAYOUT_FIELDS = ("seq_row0", "seq_len", "row_lo", "row_hi", "row_tok", "tile_kv", "cls_ctx", "cls_x", "total")
 
 
 def lib_path() -> Path:

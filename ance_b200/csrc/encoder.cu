@@ -2002,6 +2002,23 @@ extern "C" int ance_dbg_train_layout(ance_encoder_t e, int B, int L, size_t* out
   return ANCE_OK;
 }
 
+extern "C" int ance_dbg_train_layout_packed(ance_encoder_t e, const int32_t* lens_host, int B, int L, size_t* out,
+                                            int* n_tiles) {
+  const char* fn = "ance_dbg_train_layout_packed";
+  ANCE_REQUIRE(e != nullptr && out != nullptr && n_tiles != nullptr, "%s: null argument", fn);
+  PackPlan plan;
+  if (const int rc = plan_train_packed(e, lens_host, B, L, plan, fn)) return rc;
+  const TrainLayout t = train_layout(e->cfg, B, L, plan.n_tiles);
+  const PackedLayout p = packed_layout(e->cfg, B, L, plan.n_tiles);
+  static_assert(sizeof(PackedLayout) == 9 * sizeof(size_t), "ance_dbg_train_layout_packed lists every field");
+  const size_t f[kTrainLayoutFields + 9] = {t.ids, t.kbias, t.layers, t.per_layer, t.x_in, t.qkv, t.ctx, t.t1, t.x1, t.u,
+                                            t.ff, t.t2, t.x_final, t.head_in, t.total, p.seq_row0, p.seq_len, p.row_lo,
+                                            p.row_hi, p.row_tok, p.tile_kv, p.cls_ctx, p.cls_x, p.total};
+  memcpy(out, f, sizeof(f));
+  *n_tiles = plan.n_tiles;
+  return ANCE_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // test hooks: the encoder's own GEMM, attention and LayerNorm launches on caller buffers
 // ------------------------------------------------------------------------------------------------

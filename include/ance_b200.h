@@ -433,6 +433,14 @@ int ance_dbg_attention_backward_packed(int fmt, const void* qkv_dev, const float
  * u, ff [., ffn].  In the pruned last layer T1, X1, U, FF and T2 are compact: row b is sequence b's CLS row (B rows used);
  * CTX keeps its B * L rows (the CLS rows are read at pitch L * hidden); X_in and QKV are full. */
 int ance_dbg_train_layout(ance_encoder_t enc, int B, int L, size_t* out);
+/* Host-only: the workspace ance_encoder_forward_train_packed fills for the prefix lengths lens_host[B] of a [B, L] batch,
+ * planned exactly as that call plans it (the handle's current "varlen_align"; the same refusals).  *n_tiles = the plan's
+ * tiles, M = n_tiles * 128 packed rows; out[24] = the 15 fields of ance_dbg_train_layout for M rows (ids stays the dense
+ * [B * L]; kbias and every per-layer slot hold M rows, the pruned last layer's compact slots B), then seq_row0 [B],
+ * seq_len [B], row_lo, row_hi, row_tok [M] int32 (row_tok: the dense token b L + i of each row, -1 for a row of no
+ * sequence), tile_kv [n_tiles] int2, cls_ctx, cls_x [B, hidden] 16-bit (the last layer's CTX and X_in rows at seq_row0)
+ * and the total size. */
+int ance_dbg_train_layout_packed(ance_encoder_t enc, const int32_t* lens_host, int B, int L, size_t* out, int* n_tiles);
 /* Read-only copy of what a flat-IP index holds for the exactness certificate, into dst (host or device memory; the
  * stream is synchronised).  n_bytes must be the item's exact size, else ANCE_ERR_INVALID, as is an item the index does
  * not hold (no search since rows were added or the format changed; ndelta of a device index).  Items:

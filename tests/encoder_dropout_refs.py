@@ -271,23 +271,48 @@ def _site_bwd(dT, eT, m, s, perturb):
     return a, eT * mm * sb + _U32 * a.abs()
 
 
-def masked_layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, fmt, hm_out, hm_ffn, am, s, perturb=None):
+def packed_hidden_mask(seed: int, site: int, layer: int, row_tok, H: int, p: float, perturb=None) -> np.ndarray:
+    """0 / 1 mask [M, H] of a hidden site over the rows of a packed plan: row r has token row_tok[r]'s mask (a row of no
+    sequence, row_tok -1, gets 0: its gradient is 0 whatever the mask).  perturb "hidden_mask_by_row" keys the mask by
+    the row index r instead."""
+    tok = np.asarray(row_tok, dtype=np.int64)
+    keys = np.arange(len(tok)) if perturb == "hidden_mask_by_row" else np.maximum(tok, 0)
+    return hidden_mask(seed, site, layer, keys, H, p) * (tok >= 0)[:, None]
+
+
+def packed_attn_masks(seed: int, layer: int, B: int, heads: int, L: int, p: float, seq_row0=None, perturb=None):
+    """[B, heads, L, L] 0 / 1: the dense batch's masks (attn_masks), which a packed plan uses too.  perturb
+    "attn_mask_from_tile": the (query, key) counters of sequence b start at its first row's offset in its tile,
+    seq_row0[b] mod 128, instead of 0."""
+    if perturb != "attn_mask_from_tile":
+        return attn_masks(seed, layer, B, heads, L, p)
+    out = np.empty((B, heads, L, L))
+    for b in range(B):
+        o = int(seq_row0[b]) % 128
+        for h in range(heads):
+            out[b, h] = attn_mask(seed, layer, b, h, heads, L + o, p, queries=np.arange(L) + o)[:, o:o + L]
+    return out
+
+
+def masked_layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, fmt, hm_out, hm_ffn, am, s, perturb=None,
+                         plan=None, exact=False):
     """encoder_layer_refs.layer_bwd_ref with dropout: hm_out / hm_ffn the 0 / 1 masks [Mr, H] of sites 2 / 3 (the CLS
     rows' masks in the pruned last layer), am [B, heads, L, L] site 1's, s the scale.  The residual gets the LayerNorm's
-    dT; the bias gradient, wgrad and dgrad get m o dT s."""
+    dT; the bias gradient, wgrad and dgrad get m o dT s.  plan: a packed plan, as in layer_bwd_ref (the masks then those
+    of packed_hidden_mask / packed_attn_masks); exact: no bf16 conversions, as in layer_bwd_ref."""
     import torch
 
     from tests import encoder_layer_refs as LR
-    cv = LR.to_bf16
+    cv = (lambda t: t.to(torch.float64)) if exact else LR.to_bf16
     F64 = torch.float64
     dy = dy.to(F64)
-    M = B * L
+    M = B * L if plan is None else plan[3]
     g, t = {}, {}
     (dT, g["ln2_g"], g["ln2_b"], bu), (eT, t["ln2_g"], t["ln2_b"], tu) = LR.ln_stage(act["t2"], w["ln2_g"], eps, dy,
                                                                                      torch.zeros_like(dy))
     dTm, eTm = _site_bwd(dT, eT, hm_ffn, s, perturb)
     g["ff2_b"], t["ff2_b"] = (bu, tu) if perturb == "bias_unmasked" else LR._colsum(dTm, eTm)
-    A, eA = LR._rnd(dTm, eTm, False)
+    A, eA = LR._rnd(dTm, eTm, exact)
     g["ff2_w"], t["ff2_w"] = LR._mm(A.t(), eA.t(), cv(act["ff"]))
     dF, eF = LR._mm(A, eA, cv(w["w2"]))
     G = LR.G
@@ -296,37 +321,47 @@ def masked_layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, fmt, hm_out,
     dU = dF * d
     eU = eF * (d.abs() + td) + dF.abs() * td + _U32 * (dF.abs() + eF) * (d.abs() + td)
     g["ff1_b"], t["ff1_b"] = LR._colsum(dU, eU)
-    A, eA = LR._rnd(dU, eU, False)
+    A, eA = LR._rnd(dU, eU, exact)
     g["ff1_w"], t["ff1_w"] = LR._mm(A.t(), eA.t(), cv(act["x1"]))
     dX1, eX1 = LR._mm(A, eA, cv(w["w1"]))
     dX1, eX1 = LR._add(dX1, eX1, *((dTm, eTm) if perturb == "residual_masked" else (dT, eT)))
     (dT1, g["ln1_g"], g["ln1_b"], bu), (eT1, t["ln1_g"], t["ln1_b"], tu) = LR.ln_stage(act["t1"], w["ln1_g"], eps, dX1, eX1)
     dT1m, eT1m = _site_bwd(dT1, eT1, hm_out, s, perturb)
     g["ao_b"], t["ao_b"] = (bu, tu) if perturb == "bias_unmasked" else LR._colsum(dT1m, eT1m)
-    A, eA = LR._rnd(dT1m, eT1m, False)
-    ctx = act["ctx"].reshape(B, L, -1)[:, 0] if last else act["ctx"]
+    A, eA = LR._rnd(dT1m, eT1m, exact)
+    ctx = LR.last_ctx(act, B, L, plan, perturb) if last else act["ctx"]
     g["ao_w"], t["ao_w"] = LR._mm(A.t(), eA.t(), cv(ctx))
-    dC, eC = LR._rnd(*LR._mm(A, eA, cv(w["wo"])), False)
+    dC, eC = LR._rnd(*LR._mm(A, eA, cv(w["wo"])), exact)
     H = dC.shape[1]
     if last:
         dO, eO = torch.zeros(M, H, dtype=F64, device=dC.device), torch.zeros(M, H, dtype=F64, device=dC.device)
-        dO[::L], eO[::L] = dC, eC
+        rows = slice(None, None, L) if plan is None else plan[0].to(dC.device).long()
+        dO[rows], eO[rows] = dC, eC
     else:
         dO, eO = dC, eC
-    dA, eA3 = masked_attention_stage(act["qkv"], kbias, dO, eO, B, L, heads, fmt, am, s,
-                                     perturb if perturb in ("no_mask_bwd", "no_scale_bwd", "d_unmasked", "mask_transposed") else None)
+    ap = perturb if perturb in ("no_mask_bwd", "no_scale_bwd", "d_unmasked", "mask_transposed") else None
+    stage = lambda q, kb, do, edo, B_, L_, h: masked_attention_stage(q, kb, do, edo, B_, L_, h, fmt, am, s, ap)
+    if plan is None:
+        dA, eA3 = stage(act["qkv"], kbias, dO, eO, B, L, heads)
+    else:
+        dA, eA3 = LR.packed_attention(stage, act["qkv"], kbias, dO, eO, B, L, heads, plan)
     bq, tq = LR._colsum(dA, eA3)
     g["q_b"], g["k_b"], g["v_b"] = bq[:H], bq[H:2 * H], bq[2 * H:]
     t["q_b"], t["k_b"], t["v_b"] = tq[:H], tq[H:2 * H], tq[2 * H:]
-    A, eA = LR._rnd(dA, eA3, False)
+    A, eA = LR._rnd(dA, eA3, exact)
     xt = cv(act["x_in"])
     for i, n in enumerate(("q_w", "k_w", "v_w")):
         sl = slice(i * H, (i + 1) * H)
         g[n], t[n] = LR._mm(A[:, sl].t(), eA[:, sl].t(), xt)
     dX, eX = LR._mm(A, eA, cv(w["wqkv"]))
-    rows = slice(None, None, L) if last else slice(None)
     dX, eX = dX.clone(), eX.clone()
-    dX[rows], eX[rows] = LR._add(dX[rows], eX[rows], *((dT1m, eT1m) if perturb == "residual_masked" else (dT1, eT1)))
+    res, eres = (dT1m, eT1m) if perturb == "residual_masked" else (dT1, eT1)
+    if last and plan is not None:
+        rows, keep = LR.cls_rows(B, L, M, plan, perturb, dX.device)
+        res, eres = res[keep], eres[keep]
+    else:
+        rows = slice(None, None, L) if last else slice(None)
+    dX[rows], eX[rows] = LR._add(dX[rows], eX[rows], res, eres)
     g["x_in"], t["x_in"] = dX, eX
     return g, t
 

@@ -49,6 +49,22 @@ bound rejects on their data:
   "qk_bias_swap"       the q and k bias gradients swapped
   "no_ffn_residual"    dX1 without the FFN residual (add_rows(dX1 += dT) missing)
   "head_x_pitch"       head: the wgrad reads X at pitch L H (rows b L of the buffer that starts at x_final)
+and, on a packed plan (ance_encoder_forward_train_packed; `plan` below), the packed path's own index work:
+  "cls_residual_dense_rows"  last layer: the LN1 residual lands at rows b L < M (what add_rows does without seq_row0)
+  "wo_ctx_packed_rows"       last layer: the Wo wgrad reads rows 0 .. B-1 of the packed CTX instead of cls_ctx
+  "attention_whole_tile"     L <= 128: each tile's real rows attend as one sequence (a lost per-sequence bound)
+  "position_from_row"        embeddings: position ids counted from the row's offset in its tile (embedding_stage_ref)
+  "hidden_mask_by_row"       dropout: hidden masks keyed by the packed row instead of its token
+                             (encoder_dropout_refs.packed_hidden_mask)
+  "attn_mask_from_tile"      dropout: attention mask counters (query, key) start at the tile's first row instead of the
+                             sequence's (encoder_dropout_refs.packed_attn_masks)
+
+A packed plan = (seq_row0 [B], seq_len [B], row_tok [M], M): the layers' rows are the M packed rows as the forward saved
+them (row r is the dense token row_tok[r], -1 for a row of no sequence).  Row-wise stages run on those rows unchanged, and
+column sums and weight gradients over all M of them, as the kernels do.  The attention stage gathers each sequence's
+rows to dense positions b L + i (the keys past seq_len[b] masked), runs the dense stage and scatters the result back:
+rows of no sequence, and rows past a sequence's length, get exactly 0.  In the pruned last layer the B compact rows are
+the CLS rows seq_row0[b]: the Wo wgrad reads cls_ctx and the LN1 residual goes into d X_in at seq_row0[b].
 """
 from __future__ import annotations
 
@@ -137,17 +153,73 @@ def strided_rows(flat, rows, H, pitch):
     return out
 
 
-def layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, exact=False, perturb=None):
+LOG2_MASK = -10000.0 * 1.4426950408889634   # the key bias of a padding key (log2 units)
+
+
+def plan_rows(plan, L):
+    """(packed rows, dense rows b L + i) of the tokens i < seq_len[b] of every sequence of a packed plan."""
+    row0, lens = plan[0], plan[1]
+    pr = [int(row0[b]) + torch.arange(int(lens[b])) for b in range(len(row0))]
+    dr = [b * L + torch.arange(int(lens[b])) for b in range(len(row0))]
+    return torch.cat(pr), torch.cat(dr)
+
+
+def packed_attention(stage, qkv, kbias, dout, edout, B, L, heads, plan, whole_tile=False):
+    """stage(qkv, kbias, dout, edout, B, L, heads) -> (dQKV, bound), a dense attention stage, run on the M packed rows of
+    a plan: each sequence gathered to rows b L + i (keys past its length masked), the result scattered back; rows of no
+    sequence and rows past a sequence's length get exactly 0.  whole_tile (the "attention_whole_tile" perturbation, L <=
+    128): each 128-row tile's real rows attend as one sequence."""
+    dev, M, H3 = qkv.device, plan[3], qkv.shape[1]
+    if whole_tile:
+        tok = plan[2].to(dev).long()
+        real = (tok >= 0) & ((tok % L) < plan[1].to(dev).long()[tok.clamp(min=0) // L])
+        ref, tol = stage(qkv, torch.where(real, kbias.to(F64), LOG2_MASK), dout, edout, M // 128, 128, heads)
+        return ref * real[:, None], tol * real[:, None]
+    pr, dr = (t.to(dev) for t in plan_rows(plan, L))
+    n, H = B * L, dout.shape[1]
+    q = torch.zeros(n, H3, dtype=F64, device=dev)
+    kb = torch.full((n,), LOG2_MASK, dtype=F64, device=dev)
+    do, eo = torch.zeros(n, H, dtype=F64, device=dev), torch.zeros(n, H, dtype=F64, device=dev)
+    q[dr], kb[dr], do[dr], eo[dr] = qkv[pr].to(F64), kbias[pr].to(F64), dout[pr], edout[pr]
+    ref, tol = stage(q, kb, do, eo, B, L, heads)
+    out, eout = torch.zeros(M, H3, dtype=F64, device=dev), torch.zeros(M, H3, dtype=F64, device=dev)
+    out[pr], eout[pr] = ref[dr], tol[dr]
+    return out, eout
+
+
+def last_ctx(act, B, L, plan, perturb):
+    """The rows the pruned last layer's Wo wgrad reads: the CLS rows of CTX (dense: at pitch L H; packed: cls_ctx, the
+    rows seq_row0 that the forward gathered)."""
+    ctx = act["ctx"]
+    if plan is None:
+        return ctx[:B] if perturb == "wo_ctx_pitch" else ctx.reshape(B, L, -1)[:, 0]
+    if perturb == "wo_ctx_packed_rows":
+        return ctx[:B]
+    return act["cls_ctx"] if "cls_ctx" in act else ctx[plan[0].to(ctx.device).long()]
+
+
+def cls_rows(B, L, M, plan, perturb=None, dev=None):
+    """(rows of the M-row stream, which of the B compact rows land there) of the pruned last layer's CLS rows."""
+    r = torch.arange(B, device=dev) * L
+    if plan is not None and perturb != "cls_residual_dense_rows":
+        r = plan[0].to(dev).long()
+    keep = r < M
+    return r[keep], keep
+
+
+def layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, exact=False, perturb=None, plan=None):
     """One layer of backward_impl.
 
     act: the layer's saved activations widened to fp64 — x_in [M, H], qkv [M, 3H], ctx [M, H] (M = B L) and t1, x1, u,
     ff, t2 [Mr, .] (Mr = B in the pruned last layer, whose rows are then the CLS rows, else M); kbias [M] in log2 units;
     w: wqkv [3H, H], wo [H, H], w1 [F, H], w2 [H, F] as operand_fmt values (fp64), ln1_g / ln2_g [H]; dy [Mr, H] the fp32
     upstream gradient.  exact=True skips the deterministic bf16 conversions (the exact-arithmetic chain, for autograd).
+    plan = (seq_row0, seq_len, row_tok, M): the layer ran a packed plan (see the module doc); M is then the plan's row
+    count and act may carry cls_ctx [B, H], the last layer's gathered CTX rows.
     -> (grads, bounds): dicts over LAYER_GRADS + ("x_in",), x_in the gradient into the layer input [M, H]."""
     cv = (lambda t: t.to(F64)) if exact else to_bf16
     dy = dy.to(F64)
-    M = B * L
+    M = B * L if plan is None else plan[3]
     Mr = B if last else M
     zero = lambda t: torch.zeros_like(t)
     g, t = {}, {}
@@ -173,19 +245,25 @@ def layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, exact=False, pertur
     (dT1, g["ln1_g"], g["ln1_b"], g["ao_b"]), (eT1, t["ln1_g"], t["ln1_b"], t["ao_b"]) = ln_stage(
         act["t1"], w["ln1_g"], eps, dX1, eX1)
     A, eA = _rnd(dT1, eT1, exact)
-    ctx = act["ctx"]
-    if last:
-        ctx = ctx[:B] if perturb == "wo_ctx_pitch" else ctx.reshape(B, L, -1)[:, 0]
+    ctx = last_ctx(act, B, L, plan, perturb) if last else act["ctx"]
     g["ao_w"], t["ao_w"] = _mm(A.t(), eA.t(), cv(ctx))
     dC, eC = _rnd(*_mm(A, eA, cv(w["wo"])), exact)   # dCTX is stored bf16
     H = dC.shape[1]
     if last:   # cls_only: the gradient of token 0 of every sequence, none elsewhere
         dO, eO = torch.zeros(M, H, dtype=F64, device=dC.device), torch.zeros(M, H, dtype=F64, device=dC.device)
-        dO[::L], eO[::L] = dC, eC
+        if plan is None:
+            dO[::L], eO[::L] = dC, eC
+        else:
+            r0 = plan[0].to(dC.device).long()
+            dO[r0], eO[r0] = dC, eC
     else:
         dO, eO = dC, eC
     # attention -> dQKV [M, 3H]
-    dA, eA3 = attention_stage(act["qkv"], kbias, dO, eO, B, L, heads)
+    if plan is None:
+        dA, eA3 = attention_stage(act["qkv"], kbias, dO, eO, B, L, heads)
+    else:
+        dA, eA3 = packed_attention(attention_stage, act["qkv"], kbias, dO, eO, B, L, heads, plan,
+                                   whole_tile=perturb == "attention_whole_tile")
     bq, tq = _colsum(dA, eA3)
     g["q_b"], g["k_b"], g["v_b"] = bq[:H], bq[H:2 * H], bq[2 * H:]
     t["q_b"], t["k_b"], t["v_b"] = tq[:H], tq[H:2 * H], tq[2 * H:]
@@ -197,9 +275,13 @@ def layer_bwd_ref(act, kbias, w, dy, B, L, heads, last, eps, exact=False, pertur
         s = slice(i * H, (i + 1) * H)
         g[n], t[n] = _mm(A[:, s].t(), eA[:, s].t(), xt)
     dX, eX = _mm(A, eA, cv(w["wqkv"]))
-    rows = slice(0, B) if (last and perturb == "ln1_residual_rows") else slice(None, None, L) if last else slice(None)
     dX, eX = dX.clone(), eX.clone()
-    dX[rows], eX[rows] = _add(dX[rows], eX[rows], dT1, eT1)
+    if last and plan is not None:
+        rows, keep = cls_rows(B, L, M, plan, perturb, dX.device)
+        dX[rows], eX[rows] = _add(dX[rows], eX[rows], dT1[keep], eT1[keep])
+    else:
+        rows = slice(0, B) if (last and perturb == "ln1_residual_rows") else slice(None, None, L) if last else slice(None)
+        dX[rows], eX[rows] = _add(dX[rows], eX[rows], dT1, eT1)
     g["x_in"], t["x_in"] = dX, eX
     return g, t
 
@@ -221,21 +303,39 @@ def head_bwd_ref(d_out, head_in, x_final, head_w, head_g, exact=False, perturb=N
     return g, t
 
 
-def embedding_sum(ids, word, pos, typ, pad_id, roberta, max_pos):
+def embedding_sum(ids, word, pos, typ, pad_id, roberta, max_pos, pos_shift=0):
     """E = (word[id] + pos[p]) + type[0] in the tables' precision (fp32 tables: exactly embed_sum_kernel's values)."""
-    p = G.position_ids(ids.long().cpu(), pad_id, roberta).clamp(max=max_pos - 1).to(word.device)
+    p = (G.position_ids(ids.long().cpu(), pad_id, roberta) + pos_shift).clamp(0, max_pos - 1).to(word.device)
     return (word[ids.long()] + pos[p]) + typ[0]
 
 
-def embedding_stage_ref(ids, dx0, word, pos, typ, emb_g, eps, pad_id, roberta):
+def packed_to_dense(x, row_tok, n):
+    """Rows [M, .] of a packed plan scattered to their dense tokens (row r to row_tok[r]) of an n-row zero matrix."""
+    tok = row_tok.to(x.device).long()
+    out = torch.zeros(n, x.shape[1], dtype=x.dtype, device=x.device)
+    out[tok[tok >= 0]] = x[tok >= 0]
+    return out
+
+
+def position_from_row_shift(plan, lens, B, L):
+    """pos_shift [B, L] of the "position_from_row" perturbation: token i < lens[b] of sequence b at its row's offset in
+    its tile, (seq_row0[b] + i) mod 128, instead of i."""
+    i = torch.arange(L)[None, :]
+    shift = (plan[0].long().cpu()[:, None] + i) % 128 - i
+    return torch.where(i < torch.as_tensor(lens).long()[:, None], shift, 0)
+
+
+def embedding_stage_ref(ids, dx0, word, pos, typ, emb_g, eps, pad_id, roberta, pos_shift=0):
     """d X_0 [B L, H] (slot 0) through the embedding LayerNorm into the tables.  -> (grads, bounds) over word_emb,
-    pos_emb, type_emb (row 0 = the LayerNorm's column sum of dE; the other rows get nothing), emb_ln_g, emb_ln_b."""
+    pos_emb, type_emb (row 0 = the LayerNorm's column sum of dE; the other rows get nothing), emb_ln_g, emb_ln_b.
+    dx0 holds dense rows: the caller scatters a packed plan's slot 0 to its dense tokens first (packed_to_dense).
+    pos_shift [B, L] (a perturbation) moves the position ids."""
     vocab, max_pos, H = word.shape[0], pos.shape[0], word.shape[1]
-    E = embedding_sum(ids, word, pos, typ, pad_id, roberta, max_pos).reshape(-1, H)
+    E = embedding_sum(ids, word, pos, typ, pad_id, roberta, max_pos, pos_shift).reshape(-1, H)
     dx0 = dx0.to(F64)
     (dE, dg, db, ds), (eE, tg, tb, ts) = ln_stage(E, emb_g, eps, dx0, torch.zeros_like(dx0))
     idc = ids.long().cpu()
-    dw, dp = G.embedding_grads_ref(idc, dE.cpu(), vocab, max_pos, pad_id, roberta)
+    dw, dp = G.embedding_grads_ref(idc, dE.cpu(), vocab, max_pos, pad_id, roberta, pos_shift)
     tw, tp = G.embedding_grads_tol(idc, (dE.abs() + eE).cpu(), vocab, max_pos, pad_id, roberta)
     ew, ep = G.embedding_grads_ref(idc, eE.cpu(), vocab, max_pos, pad_id, roberta)   # the scatter of the dE bound
     dt = torch.zeros(typ.shape[0], H, dtype=F64, device=dE.device)
