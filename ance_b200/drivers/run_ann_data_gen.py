@@ -175,11 +175,17 @@ def _host_index(dim: int, capacity: int, device, operand: str):
 class B200Backend:
     """Encode + search on this rank's GPU through libance_b200."""
 
-    def __init__(self, args, model, mask_mode: str = "lens"):
+    def __init__(self, args, model, mask_mode: Optional[str] = None):
+        """mask_mode: "lens": 1^len 0^(L-len) from the cache's lengths (msmarco_data.py:282); "ids": input_ids != the
+        model's `mask_pad_id` (DPR: 0, DPR_data.py:283; seeddot_nll: its pad_token_id, the mask the SEED-Encoder derives
+        itself); "nonzero": the DPR driver's name for "ids".  None: "ids" for a model with a `mask_pad_id`, else "lens"."""
         self.args = args
         self.model = model
         self.device = args.device
-        self.mask_mode = mask_mode  # "lens": 1^len 0^(L-len) (msmarco_data.py:282); "nonzero": ids != 0 (DPR_data.py:283)
+        if mask_mode is None:
+            mask_mode = "ids" if hasattr(model, "mask_pad_id") else "lens"
+        self.mask_mode = "ids" if mask_mode == "nonzero" else mask_mode
+        self.pad_id = int(getattr(model, "mask_pad_id", 0))
 
     def encode(self, cache_path: str, is_query: bool, build_index: bool = False):
         """This rank's records of one token cache -> (rows [n_rows, 768] fp32 CUDA, embedding2id int64), or
@@ -201,12 +207,12 @@ class B200Backend:
         # of B; elsewhere B has no effect on the result and the pass is filled completely (592 x 128 tokens = 592 row
         # tiles of the encoder GEMMs).
         per = max(B, (args.encode_batch_tokens // L) // B * B) if multi else max(1, args.encode_batch_tokens // L)
-        bucketed = self.mask_mode != "nonzero" and not multi and getattr(args, "length_buckets", True)
+        bucketed = self.mask_mode == "lens" and not multi and getattr(args, "length_buckets", True)
         varlen = bucketed and L <= 128 and getattr(args, "varlen", True) and hasattr(self.model, "encode_lens_varlen")
-        # MaxP documents and DPR passages / questions: the packed forward in exact mode (align 16), whose embeddings are
-        # bit-identical to the padded forward's
+        # MaxP documents and the caches masked by their ids (DPR, SEED-Encoder): the packed forward in exact mode
+        # (align 16), whose embeddings are bit-identical to the padded forward's
         packed = getattr(args, "varlen", True) and hasattr(
-            self.model, "query_emb_packed" if self.mask_mode == "nonzero" else "encode_lens_multi_chunk_packed")
+            self.model, "query_emb_packed" if self.mask_mode == "ids" else "encode_lens_multi_chunk_packed")
         if bucketed:
             per *= 8   # every length bucket of a super-batch should still fill the GPU (the encoder re-splits by tokens)
         reader = StridedBatchReader(cache, per, rank=rank, world_size=W)
@@ -238,13 +244,13 @@ class B200Backend:
                     out = stage[:ids.shape[0] * C]
                 else:
                     out = rows[pos:pos + ids.shape[0] * C]
-                if self.mask_mode == "nonzero" and packed:
+                if self.mask_mode == "ids" and packed:
                     fn = self.model.query_emb_packed if is_query else self.model.body_emb_packed
                     out.copy_(fn(ids_d, align=16, ids_host=ids))
                     i = idx.numpy()
-                elif self.mask_mode == "nonzero":
+                elif self.mask_mode == "ids":
                     fn = self.model.query_emb if is_query else self.model.body_emb
-                    out.copy_(fn(ids_d, ids_d != 0))
+                    out.copy_(fn(ids_d, ids_d != self.pad_id))
                     i = idx.numpy()
                 elif multi:
                     if packed:

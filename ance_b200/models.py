@@ -29,6 +29,7 @@ from typing import Optional
 import numpy as np
 import torch
 from torch import nn
+from transformers import PretrainedConfig
 
 from . import _lib
 
@@ -89,6 +90,10 @@ _HEAD_FIELDS = ("head_w", "head_b", "head_ln_g", "head_ln_b")
 def _param_groups(backbone: nn.Module, head: Optional[tuple]):
     """The parameters in the order of ance_encoder_weights: embeddings (5), per layer the 16 of ance_layer_weights, head
     (4, or none)."""
+    if hasattr(backbone, "kernel_params"):   # a backbone under other names (SEED-Encoder) lists its own
+        embs, layers = backbone.kernel_params()
+        hd = [] if head is None else [head[0].weight, head[0].bias, head[1].weight, head[1].bias]
+        return embs, layers, hd
     emb = backbone.embeddings
     embs = [emb.word_embeddings.weight, emb.position_embeddings.weight, emb.token_type_embeddings.weight,
             emb.LayerNorm.weight, emb.LayerNorm.bias]
@@ -120,6 +125,30 @@ def _fill(struct_cls, layer_cls, groups, ptr):
     return w, lw
 
 
+def _load_checkpoint(model: nn.Module, path: str) -> nn.Module:
+    """Load `path`'s pytorch_model.bin / model.safetensors into `model` and put it in eval() mode: tensors the model does
+    not have are ignored, a tensor it has that the checkpoint lacks raises KeyError."""
+    sd = None
+    for fn in ("pytorch_model.bin", "model.safetensors"):
+        p = os.path.join(path, fn)
+        if os.path.exists(p):
+            if fn.endswith(".bin"):
+                sd = torch.load(p, map_location="cpu", weights_only=True)
+            else:
+                from safetensors.torch import load_file
+                sd = load_file(p)
+            break
+    if sd is None:
+        raise FileNotFoundError(f"no pytorch_model.bin / model.safetensors under {path}")
+    own = model.state_dict()
+    missing = [k for k in own if k not in sd]
+    if missing:
+        raise KeyError(f"checkpoint {path} lacks {len(missing)} tensors, e.g. {missing[:3]}")
+    model.load_state_dict({k: sd[k] for k in own}, strict=True)
+    model.eval()
+    return model
+
+
 def _dev_ptr(t: torch.Tensor):
     return C.cast(C.c_void_p(t.data_ptr()), C.POINTER(C.c_float))
 
@@ -132,20 +161,20 @@ class _CudaEncoder:
         lib = _lib.load()
         self.lib = lib
         self.device = device
-        emb = backbone.embeddings
-        H = emb.word_embeddings.weight.shape[1]
-        layers = list(backbone.encoder.layer)
+        groups = _param_groups(backbone, head)
+        embs, layers, _ = groups
+        H = embs[0].shape[1]
         cfg = _lib.EncoderConfig()
         cfg.arch = arch
         cfg.n_layer = len(layers)
         cfg.hidden = H
         cfg.heads = heads
-        cfg.ffn = layers[0].intermediate.dense.weight.shape[0]
-        cfg.vocab = emb.word_embeddings.weight.shape[0]
-        cfg.max_pos = emb.position_embeddings.weight.shape[0]
-        cfg.type_vocab = emb.token_type_embeddings.weight.shape[0]
+        cfg.ffn = layers[0][10].shape[0]   # ff1_w [ffn, hidden]
+        cfg.vocab = embs[0].shape[0]
+        cfg.max_pos = embs[1].shape[0]
+        cfg.type_vocab = embs[2].shape[0]
         cfg.pad_id = pad_id
-        cfg.ln_eps = float(emb.LayerNorm.eps)
+        cfg.ln_eps = float(backbone.ln_eps if hasattr(backbone, "kernel_params") else backbone.embeddings.LayerNorm.eps)
         cfg.has_head = 1 if head is not None else 0
         cfg.operand_fmt = {"fp16": _lib.ANCE_FMT_FP16, "bf16": _lib.ANCE_FMT_BF16}[operand]
         self.operand = operand
@@ -162,7 +191,7 @@ class _CudaEncoder:
                 # ance_encoder_create reads a hidden x hidden head: any other shape would be read out of bounds
                 raise _lib.AnceError(f"the CUDA encoder's head must be Linear({H}, {H}) + LayerNorm({H}), got "
                                      f"weight {tuple(lin.weight.shape)}")
-        w, lw = _fill(_lib.EncoderWeights, _lib.LayerWeights, _param_groups(backbone, head), fp)
+        w, lw = _fill(_lib.EncoderWeights, _lib.LayerWeights, groups, fp)
         self.hidden_size = H
         self.pad_id = int(pad_id)
         self.max_tokens = int(max_tokens)
@@ -523,6 +552,32 @@ class _B200Encoder(nn.Module):
                                              self.encoder_operand))
         return cache[name][1]
 
+    def _emb_packed(self, name, backbone, arch, heads, pad_id, head, input_ids, align, ids_host):
+        """Same result as the dense forward with the mask input_ids != pad_id at the cost of the real tokens: rows whose
+        non-padding ids form a non-empty prefix go through the packed forward, the others through the dense one with
+        that mask.  The lengths are read from `ids_host` (the host copy of input_ids; copied back when not given)."""
+        self._refuse_grad("query_emb_packed / body_emb_packed")
+        if input_ids.device.type != "cuda":
+            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
+        ids = input_ids.to(torch.int32).contiguous()
+        B, L = ids.shape
+        nz = (ids_host if ids_host is not None else input_ids.cpu()).reshape(B, L) != pad_id
+        lens = nz.sum(dim=1)
+        ok = (nz == (torch.arange(L)[None, :] < lens[:, None])).all(dim=1) & (lens > 0)
+        enc = self._enc_for(name, backbone, arch, heads, pad_id, head, ids.device)
+        lens32 = lens.to(torch.int32)
+        if bool(ok.all()):
+            return enc.forward_packed(ids, lens32.to(ids.device), lens32, align=align)
+        out = torch.empty((B, enc.hidden_size), dtype=torch.float32, device=ids.device)
+        sel, rest = torch.nonzero(ok).flatten(), torch.nonzero(~ok).flatten()
+        if sel.numel():
+            sd = sel.to(ids.device)
+            out[sd] = enc.forward_packed(ids[sd].contiguous(), lens32[sel].to(ids.device), lens32[sel].contiguous(),
+                                         align=align)
+        rd = rest.to(ids.device)
+        out[rd] = enc.forward(ids[rd].contiguous(), None, (ids[rd] != pad_id).to(torch.uint8).contiguous())
+        return out
+
     def check_inputs(self) -> None:
         """Deferred input validation (keeps `body_emb`/`query_emb` asynchronous): raises if any encode since the last
         call saw a token id outside the vocabulary or a position beyond max_position_embeddings, where the reference's
@@ -602,26 +657,7 @@ class RobertaDot_NLL_LN(_B200Encoder):
         if config is None:
             from transformers import RobertaConfig
             config = RobertaConfig.from_pretrained(path)
-        model = cls(config)
-        sd = None
-        for fn in ("pytorch_model.bin", "model.safetensors"):
-            p = os.path.join(path, fn)
-            if os.path.exists(p):
-                if fn.endswith(".bin"):
-                    sd = torch.load(p, map_location="cpu", weights_only=True)
-                else:
-                    from safetensors.torch import load_file
-                    sd = load_file(p)
-                break
-        if sd is None:
-            raise FileNotFoundError(f"no pytorch_model.bin / model.safetensors under {path}")
-        own = model.state_dict()
-        missing = [k for k in own if k not in sd]
-        if missing:
-            raise KeyError(f"checkpoint {path} lacks {len(missing)} tensors, e.g. {missing[:3]}")
-        model.load_state_dict({k: sd[k] for k in own}, strict=True)  # classifier.*, pooler.*: unused (SURVEY §8 a2)
-        model.eval()
-        return model
+        return _load_checkpoint(cls(config), path)  # classifier.*, pooler.*: unused (SURVEY §8 a2)
 
     def _encoder(self, device):
         return self._enc_for("roberta", self.roberta, _lib.ANCE_ARCH_ROBERTA, self.config.num_attention_heads,
@@ -844,39 +880,18 @@ class BiEncoder(_B200Encoder):
     def body_emb(self, input_ids, attention_mask):
         return self._emb("ctx", self.ctx_model, input_ids, attention_mask)
 
-    def _emb_packed(self, name, backbone, input_ids, align, ids_host):
-        """Same result as _emb(..., input_ids != 0) (DPR_data.py:283 mask) at the cost of the real tokens: rows whose
-        nonzero ids form a non-empty prefix go through the packed forward, the others through the dense one.  The lengths
-        are read from `ids_host` (the host copy of input_ids; copied back when not given)."""
-        self._refuse_grad("query_emb_packed / body_emb_packed")
-        if input_ids.device.type != "cuda":
-            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
-        ids = input_ids.to(torch.int32).contiguous()
-        B, L = ids.shape
-        nz = (ids_host if ids_host is not None else input_ids.cpu()).reshape(B, L) != 0
-        lens = nz.sum(dim=1)
-        ok = (nz == (torch.arange(L)[None, :] < lens[:, None])).all(dim=1) & (lens > 0)
-        enc = self._enc_for(name, backbone, _lib.ANCE_ARCH_BERT, self.dims.num_attention_heads, 0, None, ids.device)
-        lens32 = lens.to(torch.int32)
-        if bool(ok.all()):
-            return enc.forward_packed(ids, lens32.to(ids.device), lens32, align=align)
-        out = torch.empty((B, self.dims.hidden_size), dtype=torch.float32, device=ids.device)
-        sel, rest = torch.nonzero(ok).flatten(), torch.nonzero(~ok).flatten()
-        if sel.numel():
-            sd = sel.to(ids.device)
-            out[sd] = enc.forward_packed(ids[sd].contiguous(), lens32[sel].to(ids.device), lens32[sel].contiguous(),
-                                         align=align)
-        rd = rest.to(ids.device)
-        out[rd] = enc.forward(ids[rd].contiguous(), None, (ids[rd] != 0).to(torch.uint8).contiguous())
-        return out
+    #: the refresher encodes DPR caches with the mask input_ids != 0 (DPR_data.py:283)
+    mask_pad_id = 0
 
     def query_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
         """query_emb(input_ids, input_ids != 0) computing the real tokens only (align: see encode_lens_packed)."""
-        return self._emb_packed("question", self.question_model, input_ids, align, ids_host)
+        return self._emb_packed("question", self.question_model, _lib.ANCE_ARCH_BERT, self.dims.num_attention_heads, 0,
+                                None, input_ids, align, ids_host)
 
     def body_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
         """body_emb(input_ids, input_ids != 0) computing the real tokens only (align: see encode_lens_packed)."""
-        return self._emb_packed("ctx", self.ctx_model, input_ids, align, ids_host)
+        return self._emb_packed("ctx", self.ctx_model, _lib.ANCE_ARCH_BERT, self.dims.num_attention_heads, 0, None,
+                                input_ids, align, ids_host)
 
     def forward(self, query_ids, attention_mask_q, input_ids_a=None, attention_mask_a=None, input_ids_b=None,
                 attention_mask_b=None):
@@ -897,31 +912,223 @@ class BiEncoder(_B200Encoder):
         return ((-torch.log_softmax(logit_matrix, dim=1)[:, 0]).mean(),)
 
 
+# ---------------------------------------------------------------------------------------------
+# seeddot_nll (SEED-Encoder)
+# ---------------------------------------------------------------------------------------------
+# configuration_seed_encoder.py:71-112: every field of the SEED-Encoder config and its default.  Only the encoder half is
+# computed here; the decoder / pretraining fields are kept so that a config.json round-trips unchanged.
+_SEED_DEFAULTS = {
+    "pad_token_id": 1, "vocab_size": 32769,
+    "encoder_layers": 12, "encoder_embed_dim": 768, "encoder_ffn_embed_dim": 3072, "encoder_attention_heads": 12,
+    "dropout": 0.1, "attention_dropout": 0.1, "activation_dropout": 0.0, "encoder_layerdrop": 0.0,
+    "max_positions": 512, "activation_fn": "gelu", "quant_noise_pq": 0.0, "quant_noise_pq_block_size": 8,
+    "train_ratio": "0.5:0.5", "decoder_atten_window": 2, "pooler_activation_fn": "tanh", "pooler_dropout": 0.0,
+    "encoder_layers_to_keep": None, "decoder_layers": 3, "decoder_embed_path": None, "decoder_embed_dim": 768,
+    "decoder_ffn_embed_dim": 3072, "decoder_attention_heads": 12, "decoder_normalize_before": True,
+    "decoder_learned_pos": True, "adaptive_softmax_cutoff": None, "adaptive_softmax_dropout": 0,
+    "share_decoder_input_output_embed": True, "share_all_embeddings": True, "no_token_positional_embeddings": False,
+    "adaptive_input": False, "no_cross_attention": False, "cross_self_attention": False, "no_scale_embedding": True,
+    "layernorm_embedding": True, "tie_adaptive_weights": True, "decoder_layers_to_keep": None,
+    "initializer_range": 0.02,
+}
+
+
+class SEEDEncoderConfig(PretrainedConfig):
+    """The SEED-Encoder checkpoint config (`model_type` "seed_encoder"), with the reference's field names and defaults.
+    `MSMarcoConfigDict["seeddot_nll"].config_class`: a SEED config.json stores only the values that differ from these
+    defaults, so it must be read through this class (RobertaConfig would fill in RoBERTa's)."""
+    model_type = "seed_encoder"
+
+    def __init__(self, **kwargs):
+        own = {k: kwargs.pop(k, v) for k, v in _SEED_DEFAULTS.items()}
+        super().__init__(**kwargs)
+        for k, v in own.items():
+            setattr(self, k, v)
+        self.decoder_output_dim = self.decoder_input_dim = self.decoder_embed_dim
+        self.decoder_layerdrop = 0
+        self.max_source_positions = self.max_target_positions = self.max_positions
+
+
+class _SeedSentenceEncoder(nn.Module):
+    """Parameter skeleton of the SEED-Encoder's `TransformerSentenceEncoder` (transformer_sentence_encoder.py:695-925)
+    under its own names and registration order, with no forward of its own.  It is the post-LN RoBERTa computation the
+    encoder kernels run (ANCE_ARCH_ROBERTA): no segment embedding (a zero type row stands in: x + 0 is exact), an
+    embedding LayerNorm, separate k / v / q / out projections, erf GELU, every LayerNorm at eps 1e-5."""
+
+    ln_eps = 1e-5   # fairseq LayerNorm default (modules.py:30)
+
+    def __init__(self, vocab, hidden, n_layer, ffn, max_pos, pad_id):
+        super().__init__()
+        self.embed_tokens = nn.Embedding(vocab, hidden, padding_idx=pad_id)
+        self.embed_positions = nn.Embedding(max_pos, hidden, padding_idx=pad_id)
+        layers = []
+        for _ in range(n_layer):
+            l = _Holder()
+            att = _Holder()
+            att.k_proj, att.v_proj, att.q_proj = _linear(hidden, hidden), _linear(hidden, hidden), _linear(hidden, hidden)
+            att.out_proj = _linear(hidden, hidden)
+            l.self_attn = att
+            l.self_attn_layer_norm = nn.LayerNorm(hidden, eps=self.ln_eps)
+            l.fc1 = _linear(hidden, ffn)
+            l.fc2 = _linear(ffn, hidden)
+            l.final_layer_norm = nn.LayerNorm(hidden, eps=self.ln_eps)
+            layers.append(l)
+        self.layers = nn.ModuleList(layers)
+        self.emb_layer_norm = nn.LayerNorm(hidden, eps=self.ln_eps)
+        # the kernels' type embedding: one zero row.  Not persistent, so state_dict() keeps the reference's keys; the
+        # gradient the backward writes for it is dropped (a buffer takes no gradient).
+        self.register_buffer("type_row", torch.zeros(1, hidden), persistent=False)
+
+    def kernel_params(self):
+        """(embeddings, layers) in the order of ance_encoder_weights / ance_layer_weights (see _param_groups)."""
+        embs = [self.embed_tokens.weight, self.embed_positions.weight, self.type_row, self.emb_layer_norm.weight,
+                self.emb_layer_norm.bias]
+        layers = []
+        for l in self.layers:
+            a = l.self_attn
+            layers.append([a.q_proj.weight, a.q_proj.bias, a.k_proj.weight, a.k_proj.bias, a.v_proj.weight, a.v_proj.bias,
+                           a.out_proj.weight, a.out_proj.bias, l.self_attn_layer_norm.weight, l.self_attn_layer_norm.bias,
+                           l.fc1.weight, l.fc1.bias, l.fc2.weight, l.fc2.bias, l.final_layer_norm.weight,
+                           l.final_layer_norm.bias])
+        return embs, layers
+
+
+class SEEDEncoderDot_NLL_LN_B200(_B200Encoder):
+    """model/models.py:201-221 (`seeddot_nll`) on the sm_90a encoder: SEED-Encoder -> CLS -> Linear(768, 768) ->
+    LayerNorm(768).  Parameter names, shapes and order are the reference's (seed_encoder.encoder.sentence_encoder.*,
+    the unused classification_heads.*, embeddingHead.*, norm.*), so pytorch_model.bin and optimizer.pt are
+    interchangeable with it.
+
+    As in the reference, the attention mask comes from the ids: keys whose id is config.pad_token_id are masked
+    (transformer_sentence_encoder.py:878) and the `attention_mask` argument is ignored.  A cache padded with another id
+    therefore attends to its padding, as the reference does.  A row made only of padding, where the reference's softmax
+    over -inf yields NaN, gets the kernels' uniform-attention vector instead."""
+
+    def __init__(self, config, model_argobj=None):
+        super().__init__()
+        self.config = config
+        self.use_mean = False if model_argobj is None else model_argobj.use_mean  # models.py:24-28
+        if self.use_mean:
+            raise NotImplementedError("use_mean=True is never registered by the reference (models.py:302-316)")
+        if config.activation_fn != "gelu":
+            raise NotImplementedError(f"activation_fn={config.activation_fn!r}: the encoder kernels compute the erf GELU "
+                                      "('gelu') only")
+        if config.quant_noise_pq > 0:
+            # q_noise > 0 also inserts a bias-free Linear after the embeddings, applied in eval mode too
+            # (transformer_sentence_encoder.py:779-786)
+            raise NotImplementedError(f"quant_noise_pq={config.quant_noise_pq}: the encoder kernels have no "
+                                      "quantization-noise embedding projection")
+        keep = config.encoder_layers_to_keep
+        n_layer = len(keep.split(",")) if keep else config.encoder_layers   # modeling_seed_encoder.py:73-74
+        H, pad = config.encoder_embed_dim, config.pad_token_id
+        se = _SeedSentenceEncoder(config.vocab_size, H, n_layer, config.encoder_ffn_embed_dim,
+                                  config.max_positions + pad + 1, pad)   # learned positions offset by pad (modules.py:289)
+        self.seed_encoder = _Holder()
+        self.seed_encoder.encoder = _Holder()
+        self.seed_encoder.encoder.sentence_encoder = se
+        self.classification_heads = _Holder()   # registered for the checkpoint's sake; query_emb never reads it
+        self.classification_heads.dense = nn.Linear(H, H)
+        self.classification_heads.out_proj = nn.Linear(H, config.num_labels)
+        self.embeddingHead = nn.Linear(H, 768)
+        self.norm = nn.LayerNorm(768)
+        self.apply(RobertaDot_NLL_LN._init_weights)   # EmbeddingMixin._init_weights (models.py:31-36)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path, *model_args, config=None, from_tf=False, cache_dir=None,
+                        **kwargs):
+        """config.json (read as SEEDEncoderConfig unless `config` is given) + pytorch_model.bin / model.safetensors.
+        Extra tensors (a pretraining checkpoint's decoder / lm_head) are ignored; a missing one raises KeyError."""
+        if from_tf:
+            raise NotImplementedError("TensorFlow checkpoints are not supported")
+        path = str(pretrained_model_name_or_path)
+        if config is None:
+            config = SEEDEncoderConfig.from_pretrained(path)
+        return _load_checkpoint(cls(config), path)
+
+    #: the refresher encodes seeddot_nll caches with the mask input_ids != pad_token_id (see the class docstring)
+    @property
+    def mask_pad_id(self) -> int:
+        return int(self.config.pad_token_id)
+
+    @property
+    def _sentence_encoder(self) -> _SeedSentenceEncoder:
+        return self.seed_encoder.encoder.sentence_encoder
+
+    def _default_dropout(self) -> tuple:
+        """dropout=True: the config's `dropout` (embeddings, attention and FFN outputs) and `attention_dropout`."""
+        return (float(self.config.dropout), float(self.config.attention_dropout))
+
+    def _encoder(self, device):
+        return self._enc_for("seed", self._sentence_encoder, _lib.ANCE_ARCH_ROBERTA, self.config.encoder_attention_heads,
+                             self.mask_pad_id, (self.embeddingHead, self.norm), device)
+
+    def query_emb(self, input_ids, attention_mask=None):
+        """CLS embedding with the mask input_ids != pad_token_id; `attention_mask` is ignored, as in the reference."""
+        if self._grad_path() and self.training:
+            for field in ("activation_dropout", "encoder_layerdrop"):
+                if getattr(self.config, field) > 0:
+                    raise NotImplementedError(f"{field}={getattr(self.config, field)}: training-mode SEED-Encoder layers "
+                                              "with it have no kernel (set it to 0, or call eval())")
+        if input_ids.device.type != "cuda":
+            raise _lib.AnceError("ance_b200 models run on an sm_90 GPU only (no CPU fallback)")
+        ids = input_ids.to(torch.int32).contiguous()
+        mask = (ids != self.mask_pad_id).to(torch.uint8)
+        enc = self._encoder(ids.device)
+        if self._grad_path():
+            return self._train_emb(enc, self._sentence_encoder, (self.embeddingHead, self.norm), ids, None, mask)
+        return enc.forward(ids, None, mask)
+
+    def body_emb(self, input_ids, attention_mask=None):
+        return self.query_emb(input_ids, attention_mask)
+
+    def query_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
+        """query_emb computing the real tokens only (align: see RobertaDot_NLL_LN.encode_lens_packed)."""
+        return self._emb_packed("seed", self._sentence_encoder, _lib.ANCE_ARCH_ROBERTA,
+                                self.config.encoder_attention_heads, self.mask_pad_id, (self.embeddingHead, self.norm),
+                                input_ids, align, ids_host)
+
+    def body_emb_packed(self, input_ids, align: int = 1, ids_host: Optional[torch.Tensor] = None):
+        return self.query_emb_packed(input_ids, align, ids_host)
+
+
 def _reference_seed_class():
-    """The reference's own stock-PyTorch class, when the reference repository is importable (its directory on sys.path,
-    as its scripts arrange with `sys.path += ['../']`)."""
+    """(the reference's own stock-PyTorch class, None) when the reference repository is importable (its directory on
+    sys.path, as its scripts arrange with `sys.path += ['../']`), else (None, the import error)."""
     try:
         from model.models import SEEDEncoderDot_NLL_LN as ref_cls   # /root/reference-style checkout
-        return ref_cls
+        return ref_cls, None
     except Exception as e:  # ImportError, or the reference's own third-party imports failing
-        raise NotImplementedError(
-            "seeddot_nll (SEED-Encoder, model/models.py:201-221) has no sm_90a kernels in ance_b200 — its backbone is a "
-            "vendored fairseq-style model outside the ANN-refresh scope (SURVEY.md par. 2.1 row 8) — and the reference's "
-            "stock module could not be imported to fall back to ({}: {}).  Put the reference checkout on sys.path to run "
-            "seeddot_nll through its own PyTorch code.".format(type(e).__name__, e)) from e
+        return None, e
+
+
+def _seed_unavailable(e):
+    return NotImplementedError(
+        "seeddot_nll (SEED-Encoder, model/models.py:201-221): the reference's stock module could not be imported "
+        "({}: {}) and no config was given.  Pass a SEEDEncoderConfig (or a checkpoint directory to from_pretrained) to "
+        "build the sm_90a model, ance_b200.models.SEEDEncoderDot_NLL_LN_B200.".format(type(e).__name__, e))
 
 
 class SEEDEncoderDot_NLL_LN:
-    """model/models.py:201-221 (`seeddot_nll`).  The registry name resolves; construction / from_pretrained FALL BACK to
-    the reference's stock PyTorch module (SURVEY.md par. 2.1 row 8): the object returned is the reference's class, so
-    `query_emb` / `body_emb` behave exactly as upstream (no GPU acceleration)."""
+    """model/models.py:201-221 (`seeddot_nll`), the registry's class.  When the reference repository is importable,
+    construction and from_pretrained return the reference's own stock-PyTorch module (no GPU acceleration); otherwise
+    they build SEEDEncoderDot_NLL_LN_B200, the same model on the sm_90a encoder, from the config or checkpoint given."""
 
     def __new__(cls, *a, **k):
-        return _reference_seed_class()(*a, **k)
+        ref, err = _reference_seed_class()
+        if ref is not None:
+            return ref(*a, **k)
+        if not a and k.get("config") is None:
+            raise _seed_unavailable(err)
+        return SEEDEncoderDot_NLL_LN_B200(*a, **k)
 
     @classmethod
     def from_pretrained(cls, *a, **k):
-        return _reference_seed_class().from_pretrained(*a, **k)
+        ref, err = _reference_seed_class()
+        if ref is not None:
+            return ref.from_pretrained(*a, **k)
+        if not a and k.get("pretrained_model_name_or_path") is None:
+            raise _seed_unavailable(err)
+        return SEEDEncoderDot_NLL_LN_B200.from_pretrained(*a, **k)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -965,7 +1172,8 @@ configs = [
     MSMarcoConfig(name="rdot_nll_multi_chunk", model=RobertaDot_CLF_ANN_NLL_MultiChunk, use_mean=False),
     MSMarcoConfig(name="dpr", model=BiEncoder, tokenizer_class=_hf("BertTokenizer"), config_class=_hf("BertConfig"),
                   use_mean=False),
-    MSMarcoConfig(name="seeddot_nll", model=SEEDEncoderDot_NLL_LN, use_mean=False),
+    MSMarcoConfig(name="seeddot_nll", model=SEEDEncoderDot_NLL_LN, use_mean=False,
+                  config_class=lambda: SEEDEncoderConfig),
 ]
 
 MSMarcoConfigDict = {cfg.name: cfg for cfg in configs}

@@ -68,6 +68,56 @@ def write_checkpoint(path: str, seed: int = 0, n_layer: int = 12, vocab: int = 5
     torch.save(random_roberta_state_dict(seed=seed, n_layer=n_layer, vocab=vocab), os.path.join(path, "pytorch_model.bin"))
 
 
+def random_seed_state_dict(seed=0, n_layer=12, hidden=768, ffn=3072, vocab=32769, max_pos=514,
+                           num_labels=2) -> Dict[str, torch.Tensor]:
+    """Seeded random weights of the reference's SEEDEncoderDot_NLL_LN (`seeddot_nll`) under its own parameter names and
+    in its registration order: what its `save_pretrained` would hold.  max_pos = max_positions + pad_token_id + 1."""
+    g = torch.Generator().manual_seed(seed)
+
+    def n(*shape, std=0.02):
+        return torch.randn(*shape, generator=g) * std
+
+    p = "seed_encoder.encoder.sentence_encoder."
+    sd = {p + "embed_tokens.weight": n(vocab, hidden), p + "embed_positions.weight": n(max_pos, hidden)}
+    for l in range(n_layer):
+        lp = f"{p}layers.{l}."
+        for nm in ("self_attn.k_proj", "self_attn.v_proj", "self_attn.q_proj", "self_attn.out_proj"):
+            sd[lp + nm + ".weight"] = n(hidden, hidden, std=0.04)
+            sd[lp + nm + ".bias"] = n(hidden, std=0.02)
+        sd[lp + "self_attn_layer_norm.weight"] = 1.0 + n(hidden, std=0.05)
+        sd[lp + "self_attn_layer_norm.bias"] = n(hidden, std=0.05)
+        sd[lp + "fc1.weight"] = n(ffn, hidden, std=0.04)
+        sd[lp + "fc1.bias"] = n(ffn, std=0.02)
+        sd[lp + "fc2.weight"] = n(hidden, ffn, std=0.04)
+        sd[lp + "fc2.bias"] = n(hidden, std=0.02)
+        sd[lp + "final_layer_norm.weight"] = 1.0 + n(hidden, std=0.05)
+        sd[lp + "final_layer_norm.bias"] = n(hidden, std=0.05)
+    sd[p + "emb_layer_norm.weight"] = 1.0 + n(hidden, std=0.05)
+    sd[p + "emb_layer_norm.bias"] = n(hidden, std=0.05)
+    sd["classification_heads.dense.weight"] = n(hidden, hidden, std=0.04)
+    sd["classification_heads.dense.bias"] = n(hidden, std=0.02)
+    sd["classification_heads.out_proj.weight"] = n(num_labels, hidden, std=0.04)
+    sd["classification_heads.out_proj.bias"] = n(num_labels, std=0.02)
+    sd["embeddingHead.weight"] = n(768, hidden, std=0.04)
+    sd["embeddingHead.bias"] = n(768, std=0.02)
+    sd["norm.weight"] = 1.0 + n(768, std=0.05)
+    sd["norm.bias"] = n(768, std=0.05)
+    return sd
+
+
+def write_seed_checkpoint(path: str, seed: int = 0, n_layer: int = 12, vocab: int = 32769, **config) -> None:
+    """A `seeddot_nll` checkpoint directory: config.json (SEEDEncoderConfig; `config` overrides its defaults) +
+    pytorch_model.bin of random_seed_state_dict."""
+    from .models import SEEDEncoderConfig
+    os.makedirs(path, exist_ok=True)
+    cfg = SEEDEncoderConfig(encoder_layers=n_layer, vocab_size=vocab, **config)
+    cfg.save_pretrained(path)
+    torch.save(random_seed_state_dict(seed=seed, n_layer=n_layer, hidden=cfg.encoder_embed_dim,
+                                      ffn=cfg.encoder_ffn_embed_dim, vocab=vocab,
+                                      max_pos=cfg.max_positions + cfg.pad_token_id + 1, num_labels=cfg.num_labels),
+               os.path.join(path, "pytorch_model.bin"))
+
+
 def write_token_cache(base_path: str, n: int, L: int, mean_len: float, sd_len: float, min_len: int, seed: int,
                       vocab: int = 50265, pad_id: int = 1, bos: int = 0, eos: int = 2, full_length: bool = False,
                       chunk: int = 1 << 18, part: int = 0, n_parts: int = 1) -> None:
