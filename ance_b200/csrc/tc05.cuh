@@ -62,11 +62,14 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
+// arrive on the barrier at the same smem offset in CTA `cta` of the cluster.  Used to hand a consumed ring stage back to
+// the producer of another CTA: the consumer's reads of the stage are wgmma reads that wgmma.wait_group has already
+// retired, so the arrive needs no ordering beyond its default .release.cta semantics.  The .release.cluster form compiles
+// to MEMBAR.ALL.GPU + CCTL.IVALL, which the MMA warps would pay on every K block (half the mainloop's rate on H100).
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
 __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity) {
