@@ -116,6 +116,34 @@ int run_dbg(const void* A, const void* B, int M, int N, int K, const float* bias
   return ANCE_OK;
 }
 
+// 128 x 256 tiles on two MMA warpgroups (tc05_gemm_wide_kernel): 16-bit output only
+template <uint32_t FMT>
+int run_dbg_wide(const void* A, const void* B, int M, int N, int K, const float* bias, const void* R, int act, void* C,
+                 float* C32, cudaStream_t st) {
+  using Ep = gemm::EpStoreWide<>;
+  ANCE_REQUIRE(C && !C32, "ance_dbg_gemm: variant 5 writes a 16-bit output only");
+  CUtensorMap tmA, tmB;
+  if (!tc05_host::make_tmap_2d_16b(&tmA, A, M, K, K, gemm::BM) ||
+      !tc05_host::make_tmap_2d_16b(&tmB, B, N, K, K, gemm::kWideBN)) {
+    ance::set_error("cuTensorMapEncodeTiled failed (M=%d N=%d K=%d)", M, N, K);
+    return ANCE_ERR_CUDA;
+  }
+  gemm::WorkShape ws = gemm::make_shape(M, N, K, gemm::kWideBN, 1, 0);
+  typename Ep::Params p;
+  memset(&p, 0, sizeof(p));
+  if (!gemm::make_store_wide_tmap(&p.tmC, C, M, N, N) ||
+      (R && !gemm::make_store_wide_tmap(&p.tmR, const_cast<void*>(R), M, N, N))) {
+    ance::set_error("cuTensorMapEncodeTiled failed for the output or residual (M=%d N=%d)", M, N);
+    return ANCE_ERR_CUDA;
+  }
+  p.bias = bias;
+  p.R = reinterpret_cast<const uint16_t*>(R);
+  p.act = act;
+  ANCE_CUDA((gemm::launch_wide<Ep, FMT>(tmA, tmB, ws, p, 0, st)));
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
 template <uint32_t FMT>
 int dispatch_dbg(int variant, const void* A, const void* B, int M, int N, int K, const float* bias, const void* R,
                  int act, void* C, float* C32, cudaStream_t st) {
@@ -125,6 +153,7 @@ int dispatch_dbg(int variant, const void* A, const void* B, int M, int N, int K,
     case 2: return run_dbg<128, 4, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
     case 3: return run_dbg<64, 6, 2, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
     case 4: return run_dbg<64, 6, 1, FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
+    case 5: return run_dbg_wide<FMT>(A, B, M, N, K, bias, R, act, C, C32, st);
     default: ance::set_error("ance_dbg_gemm: unknown variant %d", variant); return ANCE_ERR_INVALID;
   }
 }

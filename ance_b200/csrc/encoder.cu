@@ -526,10 +526,51 @@ int gelu_form() {
 // (see gelu_form).  128 x 128 tile per CTA (the wgmma warpgroup holds the whole tile in registers: 128 fp32 accumulators
 // per thread), 4 operand stages, 4 epilogue warps reading the shared accumulator tile while the next tile is computed.
 // kDrop: dropout of the bias output before the residual (EpStore), site and mask rows as *dc says
+//
+// A call with a 16-bit output only, no activation and no dropout, large enough that its 128 x 256 tiles fill the card
+// several times over, runs tc05_gemm_wide_kernel instead (two MMA warpgroups on one 128 x 256 tile; bit-identical
+// outputs, see linear_wide).
+template <uint32_t FMT>
+int linear_wide(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
+                const uint16_t* R, uint16_t* C, cudaStream_t st, int cls, size_t ldr) {
+  using Ep = gemm::EpStoreWide<FMT>;
+  CUtensorMap tmA, tmB;
+  if (!tc05_host::make_tmap_2d_16b(&tmA, A, M, K, lda, gemm::BM) ||
+      !tc05_host::make_tmap_2d_16b(&tmB, W, N, K, K, gemm::kWideBN)) {
+    ance::set_error("encoder: cuTensorMapEncodeTiled failed (M=%d N=%d K=%d)", M, N, K);
+    return ANCE_ERR_CUDA;
+  }
+  const gemm::WorkShape ws = gemm::make_shape(M, N, K, gemm::kWideBN, 1, 0);
+  typename Ep::Params p;
+  memset(&p, 0, sizeof(p));
+  if (!gemm::make_store_wide_tmap(&p.tmC, C, M, N, N) ||
+      (R && !gemm::make_store_wide_tmap(&p.tmR, const_cast<uint16_t*>(R), M, N, static_cast<int>(ldr)))) {
+    ance::set_error("encoder: cuTensorMapEncodeTiled failed for the output or residual (M=%d N=%d)", M, N);
+    return ANCE_ERR_CUDA;
+  }
+  p.bias = bias;
+  p.R = R;
+  {
+    ance::ProfScope ps(cls, st);
+    ANCE_CUDA((gemm::launch_wide<Ep, FMT>(tmA, tmB, ws, p, 0, st)));
+  }
+  ance::count_launch(1);
+  return ANCE_OK;
+}
+
+// fewest 128 x 256 tiles, in waves of one tile per SM, for which a call takes linear_wide.  On an H100 at 700 W the
+// wide tile was faster at one encoder pass of the flagship (75,776 rows: 13.5 waves at N 768) and at 37,888 rows, and
+// slower at 18,944 rows and below before its epilogue was batched (DESIGN.md §4.3); smaller M is not re-measured.
+constexpr int kWideMinWaves = 10;
+
 template <uint32_t FMT, bool kDrop = false>
 int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K, const float* bias,
            const uint16_t* R, int act, uint16_t* C, float* C32, cudaStream_t st, int cls = ance::kClsGemm,
            size_t ldr = 0, const drop::Cfg* dc = nullptr) {
+  if (ldr == 0) ldr = N;
+  if (!kDrop && C && !C32 && act == 0 &&
+      (long long)((M + gemm::BM - 1) / gemm::BM) * ((N + gemm::kWideBN - 1) / gemm::kWideBN) >= (long long)kWideMinWaves * gemm::sm_count())
+    return linear_wide<FMT>(A, lda, M, W, N, K, bias, R, C, st, cls, ldr);
   constexpr int BN = 128, CG = 1, EW = 4, STAGES = 4;
   using Ep = gemm::EpStore<BN, EW, FMT, kDrop>;
   CUtensorMap tmA, tmB;
@@ -544,7 +585,6 @@ int linear(const uint16_t* A, size_t lda, int M, const uint16_t* W, int N, int K
     ance::set_error("encoder: cuTensorMapEncodeTiled failed for the output (M=%d N=%d)", M, N);
     return ANCE_ERR_CUDA;
   }
-  if (ldr == 0) ldr = N;
   if (C && R && !gemm::make_store_tmap(&p.tmR, const_cast<uint16_t*>(R), M, N, static_cast<int>(ldr))) {
     ance::set_error("encoder: cuTensorMapEncodeTiled failed for the residual (M=%d N=%d)", M, N);
     return ANCE_ERR_CUDA;

@@ -1,4 +1,5 @@
-// gemm_core.cuh — the one wgmma mainloop of this repo.
+// gemm_core.cuh — the wgmma mainloops of this repo: tc05_gemm_kernel (below) and tc05_gemm_wide_kernel (a 128 x 256
+// tile on two MMA warpgroups for the encoder's large bias / residual layers; see its own comment further down).
 //
 //   D[M,N] = A[M,K] * B[N,K]^T        A, B: 16-bit (bf16 or fp16), K-major, fp32 accumulate
 //
@@ -253,7 +254,153 @@ tc05_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 }
 
 // ------------------------------------------------------------------------------------------------
-// host-side launch helper
+// 128 x 256 tiles on two cooperating MMA warpgroups, epilogue from registers.
+//
+//   warpgroup 0  : warp 0 = TMA producer (128x64 A + 256x64 B per 48 KB stage, 3 stages); warps 1 and 2 = stagers of
+//                  the output buffer, one per MMA warpgroup; 40 registers per thread (setmaxnreg)
+//   warpgroup 1+g: rows 64g .. 64g+63 x 256 columns, one wgmma m64n256k16 per 16-wide K step (SS form, both operands
+//                  in the ring); 128 fp32 accumulators per thread, 232 registers per thread
+// Both warpgroups read the same B slice and their own half of the A slice.  Per 256 tensor clocks the wgmmas read
+// 20 KB of shared memory and TMA writes 12 KB into it (the 128x128 tile: 160 B per clock, this one 128).
+//
+// Epilogue: the warpgroup runs Ep::tile on its accumulators, reading the residual from and writing the 16-bit output
+// into its 64-row half of a 128x256 staging buffer.  Stager g then issues the TMA stores of that half and, once they
+// have read it, the residual load of the next tile, so the residual lands during the next mainloop.  Two mbarriers
+// per half: ready[g] (stager -> warpgroup: the residual has landed, or the half is free) and out[g] (warpgroup ->
+// stager: the outputs are in the half).  The tensor cores idle while the epilogue runs: it suits epilogues that are
+// a few hundred instructions per thread (bias, residual), not the GELU.
+// ------------------------------------------------------------------------------------------------
+constexpr int kWideBN = 256;
+constexpr int kWideStages = 3;
+
+template <int EP_SMEM>
+struct WideSmemPlan {
+  static constexpr int kABytes = BM * BK * 2;
+  static constexpr int kBBytes = kWideBN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kRingBytes = kWideStages * kStageBytes;
+  static constexpr int kEpOffset = kRingBytes;
+  static constexpr int kBarOffset = kEpOffset + EP_SMEM;
+  // full[STAGES] empty[STAGES] ready[2] out[2]
+  static constexpr int kBarBytes = (2 * kWideStages + 4) * 8;
+  static constexpr int kTotal = kBarOffset + kBarBytes;
+  static constexpr int kDynamicBytes = kTotal + 1024;  // slack for manual 1024-B alignment
+  static_assert(kDynamicBytes <= 232448, "GEMM shared memory exceeds 227 KB");
+};
+
+template <class Ep, uint32_t FMT>
+__global__ void __launch_bounds__(384, 1)
+tc05_gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                      const WorkShape ws, const __grid_constant__ typename Ep::Params ep) {
+  using Plan = WideSmemPlan<Ep::kSmemBytes>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Plan::kBarOffset);
+  uint64_t* empty_bar = full_bar + kWideStages;
+  uint64_t* ready_bar = empty_bar + kWideStages;
+  uint64_t* out_bar = ready_bar + 2;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const int total_work = ws.num_m_blks * ws.num_n_blks;
+  const int num_kb = (ws.K + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < kWideStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // every warp of both MMA warpgroups
+    }
+    for (int g = 0; g < 2; ++g) {
+      mbar_init(&ready_bar[g], 1);
+      mbar_init(&out_bar[g], 4);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ===================================== TMA producer =====================================
+      Ring<kWideStages> ring;
+      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int m_blk = w / ws.num_n_blks, nb = w - m_blk * ws.num_n_blks;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1, 1);
+          uint8_t* sa = smem + ring.stage * Plan::kStageBytes;
+          mbar_arrive_expect_tx(&full_bar[ring.stage], Plan::kStageBytes);
+          tma_load_2d(sa, &tmA, &full_bar[ring.stage], kb * BK, m_blk * BM, Ep::kHintA);
+          tma_load_2d(sa + Plan::kABytes, &tmB, &full_bar[ring.stage], kb * BK, nb * kWideBN, Ep::kHintB);
+          ring.advance();
+        }
+      }
+    } else if ((warp == 1 || warp == 2) && lane == 0) {
+      // ====================== stager of MMA warpgroup g's half of the output buffer ======================
+      const int g = warp - 1;
+      uint8_t* half = smem + Plan::kEpOffset + g * (Ep::kSmemBytes / 2);
+      uint32_t phase = 0;
+      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int m_blk = w / ws.num_n_blks, nb = w - m_blk * ws.num_n_blks;
+        const int row0 = m_blk * BM + 64 * g, col0 = nb * kWideBN;
+        Ep::fill(ep, ws, half, &ready_bar[g], row0, col0);
+        mbar_wait(&out_bar[g], phase, 2);
+        phase ^= 1;
+        Ep::drain(ep, ws, half, row0, col0);
+      }
+      bulk_wait_all();
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ===================================== MMA warpgroup g ====================================
+    const int g = wg - 1;
+    uint8_t* half = smem + Plan::kEpOffset + g * (Ep::kSmemBytes / 2);
+    Ring<kWideStages> ring;
+    uint32_t phase = 0;
+    auto release = [&](int stage) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    };
+    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+      const int m_blk = w / ws.num_n_blks, nb = w - m_blk * ws.num_n_blks;
+      float acc[128];
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[ring.stage], ring.phase, 3);
+        const uint32_t sa = smem_u32(smem + ring.stage * Plan::kStageBytes);
+        const uint32_t sb = sa + Plan::kABytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k)
+          wgmma_n256<FMT, 0>(acc, make_desc_k_sw128(sa + g * 64 * 128 + k * MMA_K * 2),
+                             make_desc_k_sw128(sb + k * MMA_K * 2), 1u);
+        wgmma_commit();
+        // the previous k block's wgmmas have finished reading their stage once at most one group is in flight
+        wgmma_wait<1>();
+        wgmma_fence_regs(acc);
+        if (prev_stage >= 0) release(prev_stage);
+        prev_stage = ring.stage;
+        ring.advance();
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      release(prev_stage);
+      mbar_wait(&ready_bar[g], phase, 4);
+      phase ^= 1;
+      Ep::tile(ep, ws, acc, half, nb * kWideBN);
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&out_bar[g]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// host-side launch helpers
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxDevices = 64;
 
@@ -299,6 +446,24 @@ cudaError_t launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const WorkSha
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, tmA, tmB, ws, ep);
+}
+
+// tc05_gemm_wide_kernel: tmA box {64, BM}, tmB box {64, kWideBN}, ws = make_shape(M, N, K, kWideBN, 1, 0)
+template <class Ep, uint32_t FMT>
+cudaError_t launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, const WorkShape& ws,
+                        const typename Ep::Params& ep, int max_ctas, cudaStream_t stream) {
+  using Plan = WideSmemPlan<Ep::kSmemBytes>;
+  auto kern = tc05_gemm_wide_kernel<Ep, FMT>;
+  static bool configured[kMaxDevices] = {};
+  const int dev = current_device();
+  if (!configured[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Plan::kDynamicBytes);
+    if (e != cudaSuccess) return e;
+    configured[dev] = true;
+  }
+  const int ctas = max(1, min(ws.num_m_blks * ws.num_n_blks, max_ctas > 0 ? max_ctas : sm_count()));
+  kern<<<ctas, 384, Plan::kDynamicBytes, stream>>>(tmA, tmB, ws, ep);
+  return cudaGetLastError();
 }
 
 inline WorkShape make_shape(int M, int N, int K, int BN, int CG, int n_splits /* <=0: one N block per item */) {

@@ -295,4 +295,109 @@ inline bool make_store_tmap(CUtensorMap* tm, void* C, int M, int N, int ldc) {
   return tc05_host::make_tmap_2d_16b(tm, C, M, N, ldc, BM, 64);
 }
 
+// Epilogue of tc05_gemm_wide_kernel, run from the MMA warpgroup's registers: C = act(acc + bias) + R, 16-bit output
+// (FMT) only, no dropout.  Per element it is EpStore's arithmetic in EpStore's order (acc + bias in fp32, the GELU form,
+// + the residual converted to fp32, one rounding), so the two give bit-identical outputs.  The GELU costs the tensor
+// cores its whole duration here (nothing overlaps this epilogue), so the encoder's FFN-up keeps EpStore.
+//
+// A warpgroup's 64 x 256 half of the staging buffer is four SWIZZLE_128B slabs of 64 rows x 64 columns, each the box
+// of one TMA load (residual) and one TMA store (output).  Slabs past N and halves past M are neither loaded nor stored.
+template <uint32_t FMT = tc05::kFmtBF16>
+struct EpStoreWide {
+  using A16 = act16::Act<FMT>;
+  static constexpr uint64_t kHintA = tc05::kEvictNormal;
+  static constexpr uint64_t kHintB = tc05::kEvictLast;  // weights: keep in L2
+  static constexpr int kSlabBytes = 64 * 128;
+  static constexpr int kSmemBytes = 2 * 4 * kSlabBytes;  // 128 x 256 16-bit
+
+  struct alignas(64) Params {
+    CUtensorMap tmC;         // 16-bit output [M, N], box {64, 64}, SWIZZLE_128B
+    CUtensorMap tmR;         // 16-bit residual, same box (valid when R != null)
+    const float* bias;       // [N] or null
+    const uint16_t* R;       // residual or null
+    int act;                 // as EpStore's
+  };
+
+  __device__ static int slabs(const WorkShape& ws, int row0, int col0) {
+    return row0 < ws.M ? min(4, (ws.N - col0 + 63) / 64) : 0;
+  }
+
+  // stager: the residual of the half at (row0, col0) -> the half, completing on `bar`; without one, just arrive
+  __device__ static void fill(const Params& p, const WorkShape& ws, uint8_t* half, uint64_t* bar, int row0, int col0) {
+    const int n = p.R ? slabs(ws, row0, col0) : 0;
+    if (n == 0) {
+      tc05::mbar_arrive(bar);
+      return;
+    }
+    tc05::mbar_arrive_expect_tx(bar, n * kSlabBytes);
+    for (int s = 0; s < n; ++s) tc05::tma_load_2d(half + s * kSlabBytes, &p.tmR, bar, col0 + 64 * s, row0, tc05::kEvictFirst);
+  }
+
+  // stager: the outputs in the half -> C; returns once the stores have read the half
+  __device__ static void drain(const Params& p, const WorkShape& ws, uint8_t* half, int row0, int col0) {
+    const int n = slabs(ws, row0, col0);
+    for (int s = 0; s < n; ++s) tc05::tma_store_2d(&p.tmC, half + s * kSlabBytes, col0 + 64 * s, row0);
+    tc05::bulk_commit_group();
+    tc05::bulk_wait_read_all();
+  }
+
+  // columns 8j + c, 8j + c + 1 of rows r and r + 8 (j = 8s + i) are one 32-bit word each in 16-byte chunk i of slab s;
+  // row r + 8 has row r's swizzle.  The tensor cores idle while this runs, so each slab first issues all its bias and
+  // residual loads, then does the arithmetic without branches.
+  template <int ACT>
+  __device__ __forceinline__ static void slab(const Params& p, const WorkShape& ws, const float* acc, uint8_t* sl,
+                                              int col, int r, int c) {
+    uint32_t* w0[8];
+    float2 b[8];
+    uint32_t x0[8], x1[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      w0[i] = reinterpret_cast<uint32_t*>(sl + r * 128 + ((i ^ (r & 7)) << 4) + 2 * c);
+      b[i] = (p.bias && col + 8 * i < ws.N) ? __ldg(reinterpret_cast<const float2*>(p.bias + col + 8 * i))
+                                            : make_float2(0.f, 0.f);
+      x0[i] = p.R ? *w0[i] : 0u;
+      x1[i] = p.R ? *(w0[i] + 8 * 128 / 4) : 0u;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
+      if (p.bias) {
+        v0 += b[i].x; v1 += b[i].y; v2 += b[i].x; v3 += b[i].y;
+      }
+      if constexpr (ACT == 1) {
+        gelu_erf2(v0, v1);
+        gelu_erf2(v2, v3);
+      } else if constexpr (ACT == 2) {
+        gelu_logistic2(v0, v1);
+        gelu_logistic2(v2, v3);
+      }
+      if (p.R) {
+        const float2 y0 = A16::unpack2(x0[i]), y1 = A16::unpack2(x1[i]);
+        v0 += y0.x; v1 += y0.y; v2 += y1.x; v3 += y1.y;
+      }
+      *w0[i] = A16::pack2(v0, v1);
+      *(w0[i] + 8 * 128 / 4) = A16::pack2(v2, v3);
+    }
+  }
+
+  // MMA warpgroup: accumulator fragment of m64n256 (tc05.cuh) -> outputs in the half, residual added in place
+  __device__ static void tile(const Params& p, const WorkShape& ws, const float (&acc)[128], uint8_t* half, int col0) {
+    const int t = threadIdx.x & 127;
+    const int r = 16 * (t >> 5) + ((t & 31) >> 2);
+    const int c = 2 * (t & 3);
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int col = col0 + 64 * s + c;
+      if (p.act == 1) slab<1>(p, ws, acc + 32 * s, half + s * kSlabBytes, col, r, c);
+      else if (p.act == 2) slab<2>(p, ws, acc + 32 * s, half + s * kSlabBytes, col, r, c);
+      else slab<0>(p, ws, acc + 32 * s, half + s * kSlabBytes, col, r, c);
+    }
+  }
+};
+
+// host helper: output / residual tensor map for EpStoreWide (16-bit [M, N] with row pitch ld, box 64 x 64, SW128)
+inline bool make_store_wide_tmap(CUtensorMap* tm, void* C, int M, int N, int ld) {
+  return tc05_host::make_tmap_2d_16b(tm, C, M, N, ld, 64, 64);
+}
+
 }  // namespace gemm

@@ -150,6 +150,12 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// per-thread register budget of the calling warpgroup (all 128 threads execute it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ----------------------------------------------------------------------------------------------
 // wgmma: descriptors
 // ----------------------------------------------------------------------------------------------
@@ -212,6 +218,13 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
   TC05_S32 ", "                                                                   \
   "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
   "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define TC05_R128 TC05_R64, TC05_R8(64), TC05_R8(72), TC05_R8(80), TC05_R8(88), TC05_R8(96), TC05_R8(104), TC05_R8(112), TC05_R8(120)
+#define TC05_S128                                                                               \
+  TC05_S64 ", "                                                                                 \
+  "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "            \
+  "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "            \
+  "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, " \
+  "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
 // NAME, PTX shape + types, accumulator registers, their operand strings / constraints, operand numbers of the inputs
 #define TC05_WGMMA(NAME, INSTR, NR, SLIST, RLIST, IA, IB, IP, IT)                                                     \
   template <int kTransB>                                                                                              \
@@ -221,12 +234,19 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
                  : RLIST                                                                                              \
                  : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransB));                                            \
   }
-TC05_WGMMA(wgmma_m64n128k16_bf16, "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", 64, TC05_S64, TC05_R64, "64", "65", "66", "67")
+TC05_WGMMA(wgmma_m64n256k16_bf16, "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16", 128, TC05_S128, TC05_R128, "128", "129", "130", "131")
+TC05_WGMMA(wgmma_m64n256k16_f16, "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16", 128, TC05_S128, TC05_R128, "128", "129", "130", "131")
+TC05_WGMMA(wgmma_m64n128k16_bf16,"wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", 64, TC05_S64, TC05_R64, "64", "65", "66", "67")
 TC05_WGMMA(wgmma_m64n128k16_f16, "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16", 64, TC05_S64, TC05_R64, "64", "65", "66", "67")
 TC05_WGMMA(wgmma_m64n64k16_bf16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16", 32, TC05_S32, TC05_R32, "32", "33", "34", "35")
 TC05_WGMMA(wgmma_m64n64k16_f16, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16", 32, TC05_S32, TC05_R32, "32", "33", "34", "35")
 
 // D (+)= A[smem] * B[smem], m64 x N x k16; kTransB = 1: B is MN-major
+template <uint32_t FMT, int kTransB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (FMT == kFmtBF16) wgmma_m64n256k16_bf16<kTransB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n256k16_f16<kTransB>(d, adesc, bdesc, accumulate);
+}
 template <uint32_t FMT, int kTransB>
 __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   if constexpr (FMT == kFmtBF16) wgmma_m64n128k16_bf16<kTransB>(d, adesc, bdesc, accumulate);

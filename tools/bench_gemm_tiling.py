@@ -14,7 +14,8 @@ SM clock sampled while the rounds ran.
                                       [--rounds 5] [--iters 50] [--warmup 3]
 
 Variant 0 is the tiling every encoder linear layer runs (BN 128, 4 stages, no cluster); variant 2 the same tile on 2-CTA
-clusters that share each B tile through TMA multicast (the search's coarse pass).  DESIGN.md §4.3 has the results.
+clusters that share each B tile through TMA multicast (the search's coarse pass); variant 5 the 128 x 256 tile on two
+MMA warpgroups with the epilogue from registers (the encoder's QKV, out-proj and FFN-down).  DESIGN.md §4.3 has the results.
 """
 import argparse
 import json
@@ -32,7 +33,8 @@ from tools.bench_train import ClockSampler, _smi  # noqa: E402
 
 SHAPES = {"qkv": (2304, 768, False, 0), "out": (768, 768, True, 0), "ffn1": (3072, 768, False, 2),
           "ffn2": (768, 3072, True, 0)}   # name -> (N, K, residual, act); every layer has a bias
-VARIANT_NAMES = {0: "BN128 4st CG1", 1: "BN128 3st CG1", 2: "BN128 4st CG2", 3: "BN64 6st CG2", 4: "BN64 6st CG1"}
+VARIANT_NAMES = {0: "BN128 4st CG1", 1: "BN128 3st CG1", 2: "BN128 4st CG2", 3: "BN64 6st CG2", 4: "BN64 6st CG1",
+                 5: "BN256 3st 2 MMA WG"}
 
 
 def main():
