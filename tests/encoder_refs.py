@@ -410,6 +410,89 @@ def gelu_logistic2_emulate(x: np.ndarray, coef) -> np.ndarray:
 # ------------------------------------------------------------------------------------------------
 # reporting
 # ------------------------------------------------------------------------------------------------
+WIDE_MIN_WAVES = 10   # kWideMinWaves of encoder.cu
+
+
+def wide_tiles(M: int, N: int) -> int:
+    """128 x 256 tiles of an [M, N] output."""
+    return -(-M // 128) * -(-N // 256)
+
+
+def wide_threshold(sm_count: int) -> int:
+    """Fewest wide tiles for which linear() runs a call with a 16-bit output only, act 0 and no dropout on
+    tc05_gemm_wide_kernel (encoder.cu linear(): kWideMinWaves waves of one tile per SM)."""
+    return WIDE_MIN_WAVES * sm_count
+
+
+def wide_slice_rows(N: int, threshold: int) -> int:
+    """Most rows (a multiple of 128) of an [M, N] call that stays below the threshold: the 128 x 128 tile."""
+    return (threshold - 1) // -(-N // 256) * 128
+
+
+LINEAR_WIDE_PERTURBATIONS = ("bias n+1", "residual row+1", "residual row^64", "acc col^64", "acc row^8")
+
+
+def linear_discrimination_blocked(out, A, W, bias, R, out_fmt, block_elems=1 << 23):
+    """discrimination(out, linear_ref, linear_tol, perturbed) of an act-0 linear with a 16-bit output, computed over
+    blocks of 128-aligned rows (at most ~block_elems outputs each) so that large M stays within a few GB of fp64.
+    The perturbed references are the outputs of plausible bugs of a 128 x 256 tile on two 64-row warpgroups:
+      bias n+1          bias of the next column
+      residual row+1    residual of the next row (off-by-one pitch; the last row wraps to row 0)
+      residual row^64   residual from the other warpgroup's 64-row half of the tile
+      acc col^64        accumulator columns from the neighbouring 64-column slab
+      acc row^8         accumulator rows r and r + 8 swapped (the two rows a thread holds in the wgmma fragment)
+    A partner row or column past the matrix keeps its own value.  -> (max err / bound, {name: (fraction rejected,
+    median margin, rows)}) as discrimination returns."""
+    M, N = out.shape
+    dev = out.device
+    block = max(128, block_elems // N // 128 * 128)
+    cols = torch.arange(N, device=dev)
+    col_x = torch.where((cols ^ 64) < N, cols ^ 64, cols)
+    w = W.to(F64)
+    b = None if bias is None else bias.to(F64)
+    names = [n for n in LINEAR_WIDE_PERTURBATIONS
+             if (n.startswith("bias") and bias is not None) or (n.startswith("residual") and R is not None)
+             or n.startswith("acc")]
+    err, hit, margins = 0.0, {n: 0 for n in names}, {n: [] for n in names}
+    for r0 in range(0, M, block):
+        r1 = min(M, r0 + block)
+        rows = torch.arange(r0, r1, device=dev)
+        a = A[r0:r1].to(F64)
+        acc = a @ w.T
+        r = None if R is None else R[r0:r1].to(F64)
+
+        def compose(acc_, b_, r_):
+            x_ = acc_ if b_ is None else acc_ + b_
+            return x_, (x_ if r_ is None else x_ + r_)
+
+        x, y = compose(acc, b, r)
+        tol = linear_tol(a, W, x, y, r, 0, out_fmt)
+        o = out[r0:r1].to(F64)
+        err = max(err, ((o - y).abs() / tol).max().item())
+        for n in names:
+            if n == "bias n+1":
+                p = compose(acc, torch.roll(b, -1), r)[1]
+            elif n == "residual row+1":
+                p = compose(acc, b, R[(rows + 1) % M].to(F64))[1]
+            elif n == "residual row^64":
+                p = compose(acc, b, R[torch.where((rows ^ 64) < M, rows ^ 64, rows)].to(F64))[1]
+            elif n == "acc col^64":
+                p = compose(acc[:, col_x], b, r)[1]
+            else:
+                p = compose(acc[torch.where((rows ^ 8) < M, rows ^ 8, rows) - r0], b, r)[1]
+            changed = ((p - y).abs() / tol).amax(-1) > 2.0
+            d = ((o - p).abs() / tol).amax(-1)[changed]
+            hit[n] += int((d > 1.0).sum())
+            margins[n].append(d.cpu())
+            del p
+    rep = {}
+    for n in names:
+        d = torch.cat(margins[n])
+        rep[n] = (hit[n] / d.numel() if d.numel() else float("nan"), float(d.median()) if d.numel() else float("nan"),
+                  int(d.numel()))
+    return err, rep
+
+
 def discrimination(out, ref, tol, perturbed, changed_rows=None):
     """(max |out - ref| / tol, {name: rejection}) where rejection = (fraction of the rows the perturbation changes by
     more than 2 tol on which out lies outside tol of it, median over those rows of max |out - pert| / tol, rows)."""

@@ -244,3 +244,39 @@ def test_kernel_hooks_refuse_without_gpu(lib):
     assert lib.ance_dbg_attention(0, p, 1024, 512, 12, p, None, None, None, p, None) == 2
     assert lib.ance_dbg_attention(1, p, 1024, 256, 12, p, p, p, p, p, None) == 2
     assert lib.ance_dbg_layer_norm(0, p, 1, 768, 10, 768, p, p, 1e-5, None, p, 4, None) == 2
+
+
+def test_linear_discrimination_blocked_matches_whole_matrix():
+    """The row-blocked fp64 check of the wide-tile tests gives the whole-matrix discrimination() result (bias n+1 and
+    residual row+1 through linear_ref's own perturbations), and each of its tile-layout perturbations, played back (in
+    fp64) as a kernel output, is caught: out of bound against the reference and within bound of its own perturbed
+    reference."""
+    g = torch.Generator().manual_seed(GEN_SEED + 7)
+    M, N, K, fmt = 700, 776, 64, "bf16"
+    A = R.round16(torch.randn(M, K, generator=g, dtype=torch.float64), fmt)
+    W = R.round16(torch.randn(N, K, generator=g, dtype=torch.float64) * 0.04, fmt)
+    b = torch.randn(N, generator=g).double()
+    Rs = R.round16(torch.randn(M, N, generator=g, dtype=torch.float64), fmt)
+    x, y = R.linear_ref(A, W, b, Rs)
+    tol = R.linear_tol(A, W, x, y, Rs, 0, fmt)
+    out = R.round16(y, fmt)
+    whole = R.discrimination(out, y, tol, {"bias n+1": R.linear_ref(A, W, b, Rs, bias_shift=1)[1],
+                                           "residual row+1": R.linear_ref(A, W, b, Rs, res_shift=1)[1]})
+    err, rep = R.linear_discrimination_blocked(out, A, W, b, Rs, fmt, block_elems=256 * N)   # 3 blocks, the last ragged
+    assert err == pytest.approx(whole[0], rel=1e-12) and err <= 1.0
+    assert set(rep) == set(R.LINEAR_WIDE_PERTURBATIONS)
+    for k in whole[1]:
+        assert rep[k][0] == whole[1][k][0] == 1.0 and rep[k][2] == whole[1][k][2], (k, rep[k], whole[1][k])
+        assert rep[k][1] == pytest.approx(whole[1][k][1], rel=1e-12)
+    rows, cols = torch.arange(M), torch.arange(N)
+    acc = A @ W.T
+    bugs = {"bias n+1": acc + torch.roll(b, -1) + Rs, "residual row+1": acc + b + Rs[(rows + 1) % M],
+            "residual row^64": acc + b + Rs[torch.where((rows ^ 64) < M, rows ^ 64, rows)],
+            "acc col^64": acc[:, torch.where((cols ^ 64) < N, cols ^ 64, cols)] + b + Rs,
+            "acc row^8": acc[torch.where((rows ^ 8) < M, rows ^ 8, rows)] + b + Rs}
+    for name, bad in bugs.items():
+        e, r = R.linear_discrimination_blocked(bad, A, W, b, Rs, fmt, block_elems=256 * N)
+        assert e > 1.0 and r[name][0] == 0.0 and r[name][2] >= M // 2, (name, e, r[name])
+    # without bias and residual only the accumulator perturbations apply
+    _, r = R.linear_discrimination_blocked(R.round16(acc, fmt), A, W, None, None, fmt)
+    assert set(r) == {"acc col^64", "acc row^8"} and all(v[0] == 1.0 for v in r.values())
