@@ -117,6 +117,8 @@ SIGNATURES = {
     "ance_encoder_debug_grads": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ance_lamb_step": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int, C.c_void_p, C.c_void_p]),
+    "ance_adamw_step": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
     "ance_profile_enable": (C.c_int, [C.c_int]),
     "ance_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "ance_dbg_pack_varlen": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -320,6 +320,26 @@ int ance_lamb_step(int n, float* const* p_dev, const float* const* g_dev, float*
                    const int64_t* numel, const double* hyper, int adam, float* norms_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * AdamW optimizer step  — replaces transformers 2.3.0's AdamW.step (one eager pass per parameter tensor)
+ *   reference: built at utils/dpr_utils.py:88 (run_ann_dpr.py's default --optimizer adamW), drivers/run_ann.py:86,
+ *   drivers/run_warmup.py:80
+ * One step over n contiguous fp32 device tensors p_dev[t], g_dev[t], m_dev[t], v_dev[t] as for ance_lamb_step, with
+ * hyper[5 t .. 5 t + 4] = step_size, beta1, beta2, eps, decay of the tensor: step_size = lr sqrt(1 - beta2^step) /
+ * (1 - beta1^step) with the bias correction (lr without), computed by the caller from the tensor's own step count, and
+ * decay = lr weight_decay.  Per element:
+ *   m <- beta1 m + (1 - beta1) g,  v <- beta2 v + (1 - beta2) g^2,  p <- p - step_size m / (sqrt(v) + eps),
+ *   then, only when decay > 0, p <- p - decay p (on the updated p)
+ * with the roundings of the eager fp32 step (see csrc/optim.cu).  One kernel on `stream` whatever n (none when every
+ * numel is 0), 28 bytes of traffic per element, no host synchronisation, no atomics: the same inputs give the same bits.
+ * The host arrays are consumed before the call returns.  Pointers need only 4-byte alignment (views at any offset);
+ * numel may be 0 (then the pointers may be null).  At most 512 tensors and 16 distinct (beta1, beta2, eps) per call
+ * (the table travels as kernel parameters; step_size and decay may differ for every tensor), else
+ * ANCE_ERR_UNSUPPORTED; split larger steps into several calls.  Bad arguments are rejected before anything is
+ * enqueued. */
+int ance_adamw_step(int n, float* const* p_dev, const float* const* g_dev, float* const* m_dev, float* const* v_dev,
+                    const int64_t* numel, const double* hyper, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Device-time profile by kernel class (bench.py's roofline numbers): CUDA events recorded around every
  * launch on the launch stream.  Classes: 0 encoder GEMM, 1 attention, 2 LayerNorm/embedding/gather,
  * 3 operand quantisation, 4 coarse search GEMM, 5 exact rescore, 6 exact brute force, 7-10 encoder
